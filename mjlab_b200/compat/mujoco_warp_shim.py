@@ -12,7 +12,6 @@ array — what ``sim/randomization.py:52-55`` does — which switches the engine
 from __future__ import annotations
 
 import ctypes
-import math
 from types import SimpleNamespace
 
 import torch
@@ -26,40 +25,23 @@ __b2_compat__ = True
 __version__ = "0.0-b2compat (libb2sim)"
 
 
-class _Engine:
+class _Engine(native.Engine):
+  """The engine on the current CUDA device: fields are torch tensors over device memory.  The functions below use only
+  lib / h / nworld / device / names / tensor / stream, so that a test double with that interface can stand in."""
+
   def __init__(self, mjm, nworld: int, nconmax, njmax):
     if not torch.cuda.is_available():
       raise RuntimeError("mujoco_warp (H100 engine): no CUDA device is available; there is no CPU path")
-    self.lib = native.load_library()
-    self.nworld = int(nworld)
+    lib = native.load_library()
     self.device = torch.cuda.current_device()
-    ncon = 0
-    if nconmax is not None:
-      ncon = max(16, min(96, math.ceil(nconmax / max(nworld, 1))))
-    desc, self._keep = native.make_model_desc(mjm)
-    h = ctypes.c_void_p()
     torch.cuda.synchronize(self.device)
-    native.check(self.lib.b2_create(ctypes.byref(desc), self.nworld, ncon, int(njmax or 0), self.device, ctypes.byref(h)))
-    self.h = h
-
-  def names(self, which: int) -> list[str]:
-    return [self.lib.b2_field_name(self.h, which, i).decode() for i in range(self.lib.b2_num_fields(self.h, which))]
+    super().__init__(lib, mjm, nworld, nconmax, njmax, self.device)
 
   def tensor(self, which: int, name: str) -> torch.Tensor:
-    t = native.B2Tensor()
-    native.check(self.lib.b2_get_field(self.h, which, name.encode(), ctypes.byref(t)))
-    return tensor_from_b2(t, self)
+    return tensor_from_b2(self.get_field(which, name), self)
 
   def stream(self) -> ctypes.c_void_p:
     return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
-  def __del__(self):
-    try:
-      if self.h:
-        self.lib.b2_destroy(self.h)
-        self.h = None
-    except Exception:
-      pass
 
 
 class _Struct:

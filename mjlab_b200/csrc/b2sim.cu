@@ -5,7 +5,9 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b2sim.h"
@@ -71,8 +73,6 @@ struct b2_sim {
   cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};  // off by default
   size_t smem_bytes = 0;
-  std::map<std::string, std::vector<double>> mf;  // host copy of float model arrays
-  std::map<std::string, std::vector<int>> mi;
 };
 
 static int pad4(int n) { return (n + 3) & ~3; }
@@ -169,75 +169,151 @@ __global__ void b2_order_kernel(const int* __restrict__ niter, int niter_stride,
   }
 }
 
-// inner shapes of model float fields: dims after the (broadcast) world dimension
-struct ShapeSpec { const char* name; int second; };  // second = trailing dim (0 -> 1-D)
-static const ShapeSpec kModelShapes[] = {
-    {"body_pos", 3}, {"body_quat", 4}, {"body_ipos", 3}, {"body_iquat", 4}, {"body_mass", 0},
-    {"body_subtreemass", 0}, {"body_inertia", 3}, {"body_invweight0", 2}, {"jnt_pos", 3},
-    {"jnt_axis", 3}, {"jnt_range", 2}, {"jnt_solref", 2}, {"jnt_solimp", 5}, {"jnt_margin", 0},
-    {"jnt_stiffness", 0}, {"dof_armature", 0}, {"dof_damping", 0}, {"dof_frictionloss", 0},
-    {"dof_invweight0", 0}, {"geom_size", 3}, {"geom_pos", 3}, {"geom_quat", 4},
-    {"geom_friction", 3}, {"geom_solref", 2}, {"geom_solimp", 5}, {"geom_solmix", 0},
-    {"geom_margin", 0}, {"geom_gap", 0}, {"geom_rbound", 0}, {"geom_rgba", 4}, {"site_pos", 3},
-    {"site_quat", 4}, {"actuator_gainprm", 10}, {"actuator_biasprm", 10},
-    {"actuator_ctrlrange", 2}, {"actuator_forcerange", 2}, {"actuator_gear", 0}, {"qpos0", 0}};
+// ---- model and data tables ---------------------------------------------------------------------------------------
+// Every array of the model descriptor and every Data field is named once, in one of the tables below; validation,
+// upload, field registration and lookup all read them.
 
-static FArr* model_farr(DevModel& m, const std::string& name) {
-#define F_(x) if (name == #x) return &m.x;
-  F_(body_pos) F_(body_quat) F_(body_ipos) F_(body_iquat) F_(body_mass) F_(body_subtreemass)
-  F_(body_inertia) F_(body_invweight0) F_(jnt_pos) F_(jnt_axis) F_(jnt_range) F_(jnt_solref)
-  F_(jnt_solimp) F_(jnt_margin) F_(jnt_stiffness) F_(dof_armature) F_(dof_damping)
-  F_(dof_frictionloss) F_(dof_invweight0) F_(geom_size) F_(geom_pos) F_(geom_quat)
-  F_(geom_friction) F_(geom_solref) F_(geom_solimp) F_(geom_solmix) F_(geom_margin) F_(geom_gap)
-  F_(geom_rbound) F_(geom_rgba) F_(site_pos) F_(site_quat) F_(actuator_gainprm)
-  F_(actuator_biasprm) F_(actuator_ctrlrange) F_(actuator_forcerange) F_(actuator_gear) F_(qpos0)
-#undef F_
-  return nullptr;
+// Model sizes the descriptor's arrays scale with (D_ZERO: none).
+enum Dim { D_NQ, D_NV, D_NU, D_NBODY, D_NJNT, D_NGEOM, D_NSITE, D_NSENSOR, D_NPAIR, D_NSTATIC, D_ZERO, D_NDIM };
+
+// Float model arrays: `count` x max(width, 1) fp64 values in the descriptor, fp32 on the device, shared by all worlds
+// (stride 0) until b2_expand_model_field gives one a per-world copy.  Model fields of shape (nworld, count[, width]).
+struct FloatArray { const char* name; FArr DevModel::*dev; Dim count; int width; };
+static const FloatArray kFloatArrays[] = {
+    {"body_pos", &DevModel::body_pos, D_NBODY, 3}, {"body_quat", &DevModel::body_quat, D_NBODY, 4},
+    {"body_ipos", &DevModel::body_ipos, D_NBODY, 3}, {"body_iquat", &DevModel::body_iquat, D_NBODY, 4},
+    {"body_mass", &DevModel::body_mass, D_NBODY, 0}, {"body_subtreemass", &DevModel::body_subtreemass, D_NBODY, 0},
+    {"body_inertia", &DevModel::body_inertia, D_NBODY, 3}, {"body_invweight0", &DevModel::body_invweight0, D_NBODY, 2},
+    {"jnt_pos", &DevModel::jnt_pos, D_NJNT, 3}, {"jnt_axis", &DevModel::jnt_axis, D_NJNT, 3},
+    {"jnt_range", &DevModel::jnt_range, D_NJNT, 2}, {"jnt_solref", &DevModel::jnt_solref, D_NJNT, 2},
+    {"jnt_solimp", &DevModel::jnt_solimp, D_NJNT, 5}, {"jnt_margin", &DevModel::jnt_margin, D_NJNT, 0},
+    {"jnt_stiffness", &DevModel::jnt_stiffness, D_NJNT, 0}, {"dof_armature", &DevModel::dof_armature, D_NV, 0},
+    {"dof_damping", &DevModel::dof_damping, D_NV, 0}, {"dof_frictionloss", &DevModel::dof_frictionloss, D_NV, 0},
+    {"dof_invweight0", &DevModel::dof_invweight0, D_NV, 0}, {"geom_size", &DevModel::geom_size, D_NGEOM, 3},
+    {"geom_pos", &DevModel::geom_pos, D_NGEOM, 3}, {"geom_quat", &DevModel::geom_quat, D_NGEOM, 4},
+    {"geom_friction", &DevModel::geom_friction, D_NGEOM, 3}, {"geom_solref", &DevModel::geom_solref, D_NGEOM, 2},
+    {"geom_solimp", &DevModel::geom_solimp, D_NGEOM, 5}, {"geom_solmix", &DevModel::geom_solmix, D_NGEOM, 0},
+    {"geom_margin", &DevModel::geom_margin, D_NGEOM, 0}, {"geom_gap", &DevModel::geom_gap, D_NGEOM, 0},
+    {"geom_rbound", &DevModel::geom_rbound, D_NGEOM, 0}, {"geom_rgba", &DevModel::geom_rgba, D_NGEOM, 4},
+    {"site_pos", &DevModel::site_pos, D_NSITE, 3}, {"site_quat", &DevModel::site_quat, D_NSITE, 4},
+    {"actuator_gainprm", &DevModel::actuator_gainprm, D_NU, 10},
+    {"actuator_biasprm", &DevModel::actuator_biasprm, D_NU, 10},
+    {"actuator_ctrlrange", &DevModel::actuator_ctrlrange, D_NU, 2},
+    {"actuator_forcerange", &DevModel::actuator_forcerange, D_NU, 2},
+    {"actuator_gear", &DevModel::actuator_gear, D_NU, 0}, {"qpos0", &DevModel::qpos0, D_NQ, 0}};
+
+// Integer model arrays.  The descriptor holds exactly mult x count of them (always, or only with a static grid,
+// nstatic > 0, when `with_grid`), or any number when count is D_ZERO.  Values lie in [lo, size(hi) + hi_add), unchecked
+// when lo is kAny.  `field`: callers can read the array as a Model field (1-D, shared by all worlds), in table order.
+static const long long kAny = -(1ll << 40);
+struct IntArray {
+  const char* name; const int* DevModel::*dev; Dim count = D_ZERO; bool field = false;
+  long long lo = kAny; Dim hi = D_ZERO; int hi_add = 0; int mult = 1; bool with_grid = false;
+};
+static const IntArray kIntArrays[] = {
+    {"geom_bodyid", &DevModel::geom_bodyid, D_NGEOM, true, 0, D_NBODY},
+    {"site_bodyid", &DevModel::site_bodyid, D_NSITE, true, 0, D_NBODY},
+    {"body_parentid", &DevModel::body_parentid, D_NBODY, true, 0, D_NBODY},
+    {"body_rootid", &DevModel::body_rootid, D_NBODY, true, 0, D_NBODY},
+    {"body_jntadr", &DevModel::body_jntadr, D_NBODY, false, -1, D_NJNT},
+    {"body_jntnum", &DevModel::body_jntnum, D_NBODY, false, 0, D_NJNT, 1},
+    {"body_dofadr", &DevModel::body_dofadr, D_NBODY, false, -1, D_NV},
+    {"body_dofnum", &DevModel::body_dofnum, D_NBODY, false, 0, D_NV, 1},
+    {"jnt_type", &DevModel::jnt_type, D_NJNT, true, 0, D_ZERO, 4},
+    {"jnt_qposadr", &DevModel::jnt_qposadr, D_NJNT, true, 0, D_NQ},
+    {"jnt_dofadr", &DevModel::jnt_dofadr, D_NJNT, true, 0, D_NV},
+    {"jnt_bodyid", &DevModel::jnt_bodyid, D_NJNT, false, 0, D_NBODY},
+    {"jnt_limited", &DevModel::jnt_limited, D_NJNT, false, 0, D_ZERO, 2},
+    {"dof_bodyid", &DevModel::dof_bodyid, D_NV, true, 0, D_NBODY},
+    {"dof_jntid", &DevModel::dof_jntid, D_NV, false, 0, D_NJNT},
+    {"dof_parentid", &DevModel::dof_parentid, D_NV, false, -1, D_NV},
+    {"geom_type", &DevModel::geom_type, D_NGEOM, true, 0, D_ZERO, 9},
+    {"geom_condim", &DevModel::geom_condim, D_NGEOM, true, 1, D_ZERO, 7},
+    {"geom_priority", &DevModel::geom_priority, D_NGEOM, true},
+    {"actuator_trnid", &DevModel::actuator_trnid, D_NU, true, 0, D_NJNT},
+    {"actuator_ctrllimited", &DevModel::actuator_ctrllimited, D_NU, false, 0, D_ZERO, 2},
+    {"actuator_forcelimited", &DevModel::actuator_forcelimited, D_NU, false, 0, D_ZERO, 2},
+    {"pair_geom1", &DevModel::pair_geom1, D_NPAIR, false, 0, D_NGEOM},
+    {"pair_geom2", &DevModel::pair_geom2, D_NPAIR, false, 0, D_NGEOM},
+    {"sensor_objtype", &DevModel::sensor_objtype, D_NSENSOR}, {"sensor_objid", &DevModel::sensor_objid, D_NSENSOR},
+    {"sensor_reftype", &DevModel::sensor_reftype, D_NSENSOR}, {"sensor_refid", &DevModel::sensor_refid, D_NSENSOR},
+    {"sensor_intprm", &DevModel::sensor_intprm, D_NSENSOR, false, kAny, D_ZERO, 0, 3},
+    {"sensor_adr", &DevModel::sensor_adr, D_NSENSOR, false, 0, D_ZERO, 1 << 20},
+    {"sensor_dim", &DevModel::sensor_dim, D_NSENSOR, false, 0, D_ZERO, 1 << 20},
+    {"geom_contype", &DevModel::geom_contype, D_NGEOM, false, kAny, D_ZERO, 0, 1, true},
+    {"geom_conaffinity", &DevModel::geom_conaffinity, D_NGEOM, false, kAny, D_ZERO, 0, 1, true},
+    {"static_geom", &DevModel::static_geom, D_NSTATIC, false, 0, D_NGEOM, 0, 1, true},
+    {"static_cell0", &DevModel::static_cell0, D_NSTATIC, false, 0, D_ZERO, 1 << 20, 2, true},
+    {"dyn_cgeom", &DevModel::dyn_cgeom, D_ZERO, false, 0, D_NGEOM},
+    {"grid_items", &DevModel::grid_items, D_ZERO, false, 0, D_NSTATIC}, {"grid_start", &DevModel::grid_start},
+    {"geom_dataid", &DevModel::geom_dataid}, {"mesh_vertadr", &DevModel::mesh_vertadr}, {"mesh_vertnum", &DevModel::mesh_vertnum},
+    {"hfield_adr", &DevModel::hfield_adr}, {"hfield_nrow", &DevModel::hfield_nrow}, {"hfield_ncol", &DevModel::hfield_ncol}};
+
+// Mesh and height-field assets: fp64 in the descriptor, fp32 on the device, shared by all worlds; not fields.
+struct AssetArray { const char* name; const float* DevModel::*dev; };
+static const AssetArray kAssetArrays[] = {
+    {"mesh_vert", &DevModel::mesh_vert}, {"hfield_size", &DevModel::hfield_size}, {"hfield_data", &DevModel::hfield_data}};
+
+// The descriptor's arrays, copied by b2_create and used only while it runs; the tables' arrays are looked up by
+// their DevModel member (absent arrays read as empty).
+struct HostModel {
+  std::map<std::string, std::vector<int>> i;
+  std::map<std::string, std::vector<double>> f;
+
+  template <class T> static const std::vector<T>& find(const std::map<std::string, std::vector<T>>& m, const char* k) {
+    static const std::vector<T> none;
+    auto it = m.find(k);
+    return it == m.end() ? none : it->second;
+  }
+  template <class Row, size_t N, class Member>
+  static const char* name_of(const Row (&rows)[N], Member dev) {
+    for (const Row& r : rows) if (r.dev == dev) return r.name;
+    return "";
+  }
+  const std::vector<int>& at(const int* DevModel::*a) const { return find(i, name_of(kIntArrays, a)); }
+  const std::vector<double>& at(FArr DevModel::*a) const { return find(f, name_of(kFloatArrays, a)); }
+  const std::vector<double>& at(const float* DevModel::*a) const { return find(f, name_of(kAssetArrays, a)); }
+  double scalar(const char* k) const {  // a size or option scalar, given as int32 or float64 (0 when absent)
+    const std::vector<int>& vi = find(i, k); const std::vector<double>& vf = find(f, k);
+    return !vi.empty() ? vi[0] : vf.empty() ? 0.0 : vf[0];
+  }
+};
+
+// A field of `n` values per world, `wstride` elements apart (0: shared by all worlds).  `width` > 0 splits a world's
+// values into (n / width, width), 9 into (n / 9, 3, 3) like mjwarp's mat33 arrays; `per_world`: one value per world,
+// shape (nworld,).
+static Field make_field(const char* name, void* p, int dtype, int nworld, int64_t wstride, int64_t n, int width,
+                        bool per_world) {
+  Field f;
+  f.name = name; f.ptr = p; f.dtype = dtype; f.n = n;
+  f.shape[0] = nworld; f.stride[0] = wstride;
+  if (per_world) f.ndim = 1;
+  else if (width == 9) {
+    f.ndim = 4; f.shape[1] = n / 9; f.shape[2] = 3; f.shape[3] = 3;
+    f.stride[1] = 9; f.stride[2] = 3; f.stride[3] = 1;
+  } else if (width > 0) {
+    f.ndim = 3; f.shape[1] = n / width; f.shape[2] = width; f.stride[1] = width; f.stride[2] = 1;
+  } else { f.ndim = 2; f.shape[1] = n; f.stride[1] = 1; }
+  return f;
 }
 
-static int add_data(b2_sim* s, const char* name, DArr* arr, int n, int second = 0) {
-  int stride = pad4(std::max(n, 0));
-  if (stride == 0) stride = 4;
+// A per-world Data array (DArr: float, IArr: int) of `n` values per world; see make_field for `width`, `per_world`.
+template <class A>
+struct DataArray { const char* name; A DevData::*dev; int n; int width = 0; bool per_world = false; };
+
+template <class A>
+static int add_data(b2_sim* s, const DataArray<A>& r) {
+  using T = typename std::remove_pointer<decltype(A::p)>::type;
+  const int stride = r.n > 0 ? pad4(r.n) : 4;  // rows padded to 16 B
   void* p = nullptr;
-  size_t bytes = sizeof(float) * (size_t)s->nworld * stride;
+  size_t bytes = sizeof(T) * (size_t)s->nworld * stride;
   CUDA_OK(cudaMalloc(&p, bytes));
-  CUDA_OK(cudaMemset(p, 0, bytes));
   s->allocs.push_back(p);
-  arr->p = (float*)p; arr->stride = stride; arr->n = n;
-  Field f;
-  f.name = name; f.ptr = p; f.dtype = B2_F32; f.n = n;
-  if (second == 9) {  // rotation matrices are exposed as (nworld, n, 3, 3) like mjwarp's mat33 arrays
-    f.ndim = 4; f.shape[0] = s->nworld; f.shape[1] = n / 9; f.shape[2] = 3; f.shape[3] = 3;
-    f.stride[0] = stride; f.stride[1] = 9; f.stride[2] = 3; f.stride[3] = 1;
-  } else if (second > 0) {
-    f.ndim = 3; f.shape[0] = s->nworld; f.shape[1] = n / second; f.shape[2] = second;
-    f.stride[0] = stride; f.stride[1] = second; f.stride[2] = 1;
-  } else {
-    f.ndim = 2; f.shape[0] = s->nworld; f.shape[1] = n;
-    f.stride[0] = stride; f.stride[1] = 1;
-  }
-  s->data_fields.push_back(f);
-  return 0;
-}
-static int add_idata(b2_sim* s, const char* name, IArr* arr, int n, int second = 0) {
-  int stride = pad4(std::max(n, 1));
-  void* p = nullptr;
-  size_t bytes = sizeof(int) * (size_t)s->nworld * stride;
-  CUDA_OK(cudaMalloc(&p, bytes));
   CUDA_OK(cudaMemset(p, 0, bytes));
-  s->allocs.push_back(p);
-  arr->p = (int*)p; arr->stride = stride; arr->n = n;
-  Field f;
-  f.name = name; f.ptr = p; f.dtype = B2_I32; f.n = n;
-  if (second > 0) {
-    f.ndim = 3; f.shape[0] = s->nworld; f.shape[1] = n / second; f.shape[2] = second;
-    f.stride[0] = stride; f.stride[1] = second; f.stride[2] = 1;
-  } else if (n == 1) {
-    f.ndim = 1; f.shape[0] = s->nworld; f.stride[0] = stride;
-  } else {
-    f.ndim = 2; f.shape[0] = s->nworld; f.shape[1] = n; f.stride[0] = stride; f.stride[1] = 1;
-  }
-  s->data_fields.push_back(f);
+  A& a = s->hd.*r.dev;
+  a.p = (T*)p; a.stride = stride; a.n = r.n;
+  s->data_fields.push_back(make_field(r.name, p, std::is_same<T, int>::value ? B2_I32 : B2_F32, s->nworld, stride, r.n,
+                                      r.width, r.per_world));
   return 0;
 }
 
@@ -298,135 +374,72 @@ int b2_phase_cycles(unsigned long long* out32) {
 #endif
 }
 
-// Sizes and index ranges of the model table (mjModel field names).  Returns "" when consistent.
-static std::string validate_desc(const B2ModelDesc* desc) {
-  std::map<std::string, const B2Array*> by;
+// Copies the descriptor's arrays into `h` and checks their sizes and index ranges (mjModel field names), so that a
+// malformed table never reaches the index loops.  Returns "" when consistent.
+static std::string read_desc(const B2ModelDesc* desc, HostModel& h) {
   for (int i = 0; i < desc->narray; i++) {
     const B2Array& a = desc->arrays[i];
     if (!a.name || a.n < 0 || (a.n > 0 && !a.data)) return "array without name or data";
-    if (a.dtype != B2_I32 && a.dtype != B2_F64) return std::string("array '") + a.name + "': dtype must be int32 or float64";
-    by[a.name] = &a;
+    if (a.dtype == B2_I32) h.i[a.name].assign((const int32_t*)a.data, (const int32_t*)a.data + a.n);
+    else if (a.dtype == B2_F64) h.f[a.name].assign((const double*)a.data, (const double*)a.data + a.n);
+    else return std::string("array '") + a.name + "': dtype must be int32 or float64";
   }
-  auto scalar = [&](const char* k, long long* out) -> bool {
-    auto it = by.find(k);
-    if (it == by.end() || it->second->n < 1) return false;
-    *out = it->second->dtype == B2_I32 ? ((const int32_t*)it->second->data)[0] : (long long)((const double*)it->second->data)[0];
-    return true;
+  static const char* const kSizes[D_ZERO] = {"nq", "nv", "nu", "nbody", "njnt", "ngeom", "nsite", "nsensor", "npair", "nstatic"};
+  long long size[D_NDIM] = {};
+  for (int k = 0; k < D_ZERO; k++) {
+    if (k != D_NSTATIC && HostModel::find(h.i, kSizes[k]).empty() && HostModel::find(h.f, kSizes[k]).empty())
+      return "missing size scalar (nq nv nu nbody njnt ngeom nsite nsensor npair)";
+    size[k] = (long long)h.scalar(kSizes[k]);
+    if (size[k] < (k == D_NQ || k == D_NV || k == D_NBODY ? 1 : 0)) return "negative or zero model size";
+  }
+  // an array of exactly n values of `dtype`, with int values in [lo, hi) unless lo is kAny ("" when it is)
+  auto require = [&](const char* name, int dtype, long long n, long long lo, long long hi) -> std::string {
+    const bool is_int = h.i.count(name) > 0;
+    long long have = is_int ? h.i.at(name).size() : HostModel::find(h.f, name).size();
+    if (have != n) return std::string("array '") + name + "' has " + std::to_string(have) + " elements, expected " + std::to_string(n);
+    if (n == 0) return "";
+    if (is_int != (dtype == B2_I32)) return std::string("array '") + name + "' has the wrong dtype";
+    if (is_int && lo != kAny)
+      for (int v : h.i.at(name))
+        if (v < lo || v >= hi) return std::string("array '") + name + "' holds an index out of range";
+    return "";
   };
-  long long nq, nv, nu, nbody, njnt, ngeom, nsite, nsensor, npair, nstatic = 0;
-  if (!scalar("nq", &nq) || !scalar("nv", &nv) || !scalar("nu", &nu) || !scalar("nbody", &nbody) || !scalar("njnt", &njnt) ||
-      !scalar("ngeom", &ngeom) || !scalar("nsite", &nsite) || !scalar("nsensor", &nsensor) || !scalar("npair", &npair))
-    return "missing size scalar (nq nv nu nbody njnt ngeom nsite nsensor npair)";
-  scalar("nstatic", &nstatic);
-  if (nq < 1 || nv < 1 || nbody < 1 || nu < 0 || njnt < 0 || ngeom < 0 || nsite < 0 || nsensor < 0 || npair < 0 || nstatic < 0)
-    return "negative or zero model size";
-  struct Req { const char* name; int dtype; long long n; long long lo, hi; };  // index range checked for lo <= v < hi
-  const long long NO = -(1ll << 40);
-  std::vector<Req> req = {
-    {"body_parentid", B2_I32, nbody, 0, nbody}, {"body_rootid", B2_I32, nbody, 0, nbody}, {"body_jntadr", B2_I32, nbody, -1, njnt},
-    {"body_jntnum", B2_I32, nbody, 0, njnt + 1}, {"body_dofadr", B2_I32, nbody, -1, nv}, {"body_dofnum", B2_I32, nbody, 0, nv + 1},
-    {"jnt_type", B2_I32, njnt, 0, 4}, {"jnt_qposadr", B2_I32, njnt, 0, nq}, {"jnt_dofadr", B2_I32, njnt, 0, nv},
-    {"jnt_bodyid", B2_I32, njnt, 0, nbody}, {"jnt_limited", B2_I32, njnt, 0, 2}, {"dof_bodyid", B2_I32, nv, 0, nbody},
-    {"dof_jntid", B2_I32, nv, 0, njnt}, {"dof_parentid", B2_I32, nv, -1, nv}, {"geom_type", B2_I32, ngeom, 0, 9},
-    {"geom_bodyid", B2_I32, ngeom, 0, nbody}, {"geom_condim", B2_I32, ngeom, 1, 7}, {"geom_priority", B2_I32, ngeom, NO, -NO},
-    {"site_bodyid", B2_I32, nsite, 0, nbody}, {"actuator_trnid", B2_I32, nu, 0, njnt},
-    {"actuator_ctrllimited", B2_I32, nu, 0, 2}, {"actuator_forcelimited", B2_I32, nu, 0, 2},
-    {"pair_geom1", B2_I32, npair, 0, ngeom}, {"pair_geom2", B2_I32, npair, 0, ngeom},
-    {"sensor_objtype", B2_I32, nsensor, NO, -NO}, {"sensor_objid", B2_I32, nsensor, NO, -NO}, {"sensor_reftype", B2_I32, nsensor, NO, -NO},
-    {"sensor_refid", B2_I32, nsensor, NO, -NO}, {"sensor_intprm", B2_I32, 3 * nsensor, NO, -NO}, {"sensor_adr", B2_I32, nsensor, 0, 1 << 20},
-    {"sensor_dim", B2_I32, nsensor, 0, 1 << 20},
-    {"body_pos", B2_F64, 3 * nbody}, {"body_quat", B2_F64, 4 * nbody}, {"body_ipos", B2_F64, 3 * nbody}, {"body_iquat", B2_F64, 4 * nbody},
-    {"body_mass", B2_F64, nbody}, {"body_subtreemass", B2_F64, nbody}, {"body_inertia", B2_F64, 3 * nbody}, {"body_invweight0", B2_F64, 2 * nbody},
-    {"jnt_pos", B2_F64, 3 * njnt}, {"jnt_axis", B2_F64, 3 * njnt}, {"jnt_range", B2_F64, 2 * njnt}, {"jnt_solref", B2_F64, 2 * njnt},
-    {"jnt_solimp", B2_F64, 5 * njnt}, {"jnt_margin", B2_F64, njnt}, {"jnt_stiffness", B2_F64, njnt}, {"dof_armature", B2_F64, nv},
-    {"dof_damping", B2_F64, nv}, {"dof_frictionloss", B2_F64, nv}, {"dof_invweight0", B2_F64, nv}, {"geom_size", B2_F64, 3 * ngeom},
-    {"geom_pos", B2_F64, 3 * ngeom}, {"geom_quat", B2_F64, 4 * ngeom}, {"geom_friction", B2_F64, 3 * ngeom}, {"geom_solref", B2_F64, 2 * ngeom},
-    {"geom_solimp", B2_F64, 5 * ngeom}, {"geom_solmix", B2_F64, ngeom}, {"geom_margin", B2_F64, ngeom}, {"geom_gap", B2_F64, ngeom},
-    {"geom_rbound", B2_F64, ngeom}, {"geom_rgba", B2_F64, 4 * ngeom}, {"site_pos", B2_F64, 3 * nsite}, {"site_quat", B2_F64, 4 * nsite},
-    {"actuator_gainprm", B2_F64, 10 * nu}, {"actuator_biasprm", B2_F64, 10 * nu}, {"actuator_ctrlrange", B2_F64, 2 * nu},
-    {"actuator_forcerange", B2_F64, 2 * nu}, {"actuator_gear", B2_F64, nu}, {"qpos0", B2_F64, nq},
-  };
-  if (nstatic > 0) {
-    req.push_back({"geom_contype", B2_I32, ngeom, NO, -NO});
-    req.push_back({"geom_conaffinity", B2_I32, ngeom, NO, -NO});
-    req.push_back({"static_geom", B2_I32, nstatic, 0, ngeom});
-    req.push_back({"static_cell0", B2_I32, 2 * nstatic, 0, 1 << 20});
-    req.push_back({"grid_params", B2_F64, 5});
+  std::string why;
+  auto require_int = [&](const IntArray& r) { return require(r.name, B2_I32, r.mult * size[r.count], r.lo, size[r.hi] + r.hi_add); };
+  for (const IntArray& r : kIntArrays)
+    if (r.count != D_ZERO && !r.with_grid && !(why = require_int(r)).empty()) return why;
+  for (const FloatArray& r : kFloatArrays)
+    if (!(why = require(r.name, B2_F64, std::max(r.width, 1) * size[r.count], kAny, 0)).empty()) return why;
+  if (size[D_NSTATIC] > 0) {
+    for (const IntArray& r : kIntArrays)
+      if (r.with_grid && !(why = require_int(r)).empty()) return why;
+    if (!(why = require("grid_params", B2_F64, 5, kAny, 0)).empty()) return why;
   }
-  for (const Req& r : req) {
-    auto it = by.find(r.name);
-    long long have = it == by.end() ? 0 : it->second->n;
-    if (have != r.n) return std::string("array '") + r.name + "' has " + std::to_string(have) + " elements, expected " + std::to_string(r.n);
-    if (r.n == 0) continue;
-    if (it->second->dtype != r.dtype) return std::string("array '") + r.name + "' has the wrong dtype";
-    if (r.dtype == B2_I32 && r.lo != NO) {
-      const int32_t* v = (const int32_t*)it->second->data;
-      for (long long i = 0; i < r.n; i++)
-        if (v[i] < r.lo || v[i] >= r.hi) return std::string("array '") + r.name + "' holds an index out of range";
-    }
+  for (const IntArray& r : kIntArrays) {  // optional index arrays: checked when present
+    if (r.count != D_ZERO || r.lo == kAny || (!h.i.count(r.name) && !h.f.count(r.name))) continue;
+    if (!h.i.count(r.name)) return std::string("array '") + r.name + "' has the wrong dtype";
+    if (!(why = require(r.name, B2_I32, h.i.at(r.name).size(), r.lo, size[r.hi] + r.hi_add)).empty()) return why;
   }
-  for (const char* k : {"dyn_cgeom", "grid_items"}) {
-    auto it = by.find(k);
-    if (it == by.end()) continue;
-    if (it->second->dtype != B2_I32) return std::string("array '") + k + "' has the wrong dtype";
-    long long hi = std::string(k) == "dyn_cgeom" ? ngeom : nstatic;
-    const int32_t* v = (const int32_t*)it->second->data;
-    for (long long i = 0; i < it->second->n; i++)
-      if (v[i] < 0 || v[i] >= hi) return std::string("array '") + k + "' holds an index out of range";
-  }
-  {  // parents precede children (the kinematic walks and the factorisation schedule rely on it)
-    const int32_t* bp = (const int32_t*)by["body_parentid"]->data;
-    for (long long b = 1; b < nbody; b++) if (bp[b] >= b) return "body_parentid: parents must precede children";
-    const int32_t* dp = (const int32_t*)by["dof_parentid"]->data;
-    for (long long d = 0; d < nv; d++) if (dp[d] >= d) return "dof_parentid: parents must precede children";
-  }
+  // parents precede children (the kinematic walks and the factorisation schedule rely on it)
+  const std::vector<int>& bp = h.at(&DevModel::body_parentid);
+  for (size_t b = 1; b < bp.size(); b++) if (bp[b] >= (int)b) return "body_parentid: parents must precede children";
+  const std::vector<int>& dp = h.at(&DevModel::dof_parentid);
+  for (size_t d = 0; d < dp.size(); d++) if (dp[d] >= (int)d) return "dof_parentid: parents must precede children";
   return "";
 }
 
-int b2_create(const B2ModelDesc* desc, int nworld, int ncon_per_world, int njmax, int cuda_device,
-              b2_sim** out) {
-  if (!desc || !out || nworld <= 0) return fail("b2_create: bad arguments");
-  {
-    std::string why = validate_desc(desc);  // host-only: a malformed table must not reach the index loops
-    if (!why.empty()) return fail("b2_create: " + why);
-  }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-    return fail("b2_create: no CUDA device available (this library has no CPU path)");
-  if (cuda_device < 0 || cuda_device >= ndev) return fail("b2_create: bad cuda_device");
-  DeviceGuard guard(cuda_device);
-  b2_sim* s = new b2_sim();
-  s->device = cuda_device;
-  s->nworld = nworld;
-  for (int i = 0; i < desc->narray; i++) {
-    const B2Array& a = desc->arrays[i];
-    if (a.dtype == B2_I32) {
-      s->mi[a.name] = std::vector<int>((const int32_t*)a.data, (const int32_t*)a.data + a.n);
-    } else if (a.dtype == B2_F64) {
-      s->mf[a.name] = std::vector<double>((const double*)a.data, (const double*)a.data + a.n);
-    } else {
-      delete s;
-      return fail("b2_create: unsupported array dtype");
-    }
-  }
-  auto geti = [&](const char* k) -> int {
-    if (s->mi.count(k)) return s->mi[k].empty() ? 0 : s->mi[k][0];
-    if (s->mf.count(k)) return (int)s->mf[k][0];
-    return 0;
-  };
-  auto getf = [&](const char* k) -> double {
-    if (s->mf.count(k)) return s->mf[k][0];
-    if (s->mi.count(k)) return s->mi[k][0];
-    return 0.0;
-  };
-  DevModel& m = s->hm;
+// ---- b2_create, stage by stage: each stage returns non-zero (message set) to refuse the model -------------------
+
+// Sizes, solver options and capacities of the model.
+static int read_model(const B2ModelDesc* desc, int ncon_per_world, int njmax, const HostModel& h, DevModel& m) {
+  auto geti = [&](const char* k) { return (int)h.scalar(k); };
   memset(&m, 0, sizeof(m));
   m.nq = geti("nq"); m.nv = geti("nv"); m.nu = geti("nu"); m.nbody = geti("nbody");
   m.njnt = geti("njnt"); m.ngeom = geti("ngeom"); m.nsite = geti("nsite");
   m.nsensor = geti("nsensor"); m.nsensordata = geti("nsensordata"); m.npair = geti("npair");
   m.ntri = m.nv * (m.nv + 1) / 2;
-  if (m.nv > 64 || m.nbody > 64) { delete s; return fail("b2_create: nv and nbody must be <= 64"); }
-  if (m.nv < 1) { delete s; return fail("b2_create: model has no degrees of freedom"); }
+  if (m.nv > 64 || m.nbody > 64) return fail("b2_create: nv and nbody must be <= 64");
+  if (m.nv < 1) return fail("b2_create: model has no degrees of freedom");
   m.integrator = geti("opt_integrator"); m.iterations = geti("opt_iterations");
   m.ls_iterations = geti("opt_ls_iterations"); m.debug = 8 | 16 | 32;  // bit 3: relative-step stop of the line search; bit 4: shifted warm start after a control
                          // change; bit 5: the line search evaluates its slope at 0 (off: grad . search and a first trial
@@ -435,23 +448,33 @@ int b2_create(const B2ModelDesc* desc, int nworld, int ncon_per_world, int njmax
   m.newton_small = 1e-10f;
   m.ls_rtol = 1e-3f;  // line search stops once the slope is 1e-3 of its value at 0 (emulated bench workload: 7.0 -> 3.4
                       // evaluations per Newton iteration, iteration count unchanged: 4.665 -> 4.67)
-  m.timestep = (float)getf("opt_timestep"); m.tolerance = (float)getf("opt_tolerance");
-  m.ls_tolerance = (float)getf("opt_ls_tolerance"); m.impratio = (float)getf("opt_impratio");
-  m.meaninertia = (float)getf("stat_meaninertia");
+  m.timestep = (float)h.scalar("opt_timestep"); m.tolerance = (float)h.scalar("opt_tolerance");
+  m.ls_tolerance = (float)h.scalar("opt_ls_tolerance"); m.impratio = (float)h.scalar("opt_impratio");
+  m.meaninertia = (float)h.scalar("stat_meaninertia");
   for (int k = 0; k < 3; k++) m.gravity[k] = (float)desc->gravity[k];
-  if (geti("opt_cone") != 0) { delete s; return fail("b2_create: only pyramidal cones are supported"); }
+  if (geti("opt_cone") != 0) return fail("b2_create: only pyramidal cones are supported");
   m.solver = geti("opt_solver");
-  if (m.solver != SOL_NEWTON_ && m.solver != SOL_CG_) {
-    delete s;
+  if (m.solver != SOL_NEWTON_ && m.solver != SOL_CG_)
     return fail("b2_create: solver must be Newton or CG (PGS works on the dual problem and is not implemented)");
-  }
   m.maxcon = ncon_per_world > 0 ? std::min(ncon_per_world, 255) : 48;
   m.njmax = njmax > 0 ? njmax : 300;
+  // supported sensor set: contact sensors with data in {found,force,dist,pos,normal}, reduce none/netforce
+  const std::vector<int>& intprm = h.at(&DevModel::sensor_intprm);
+  for (int i = 0; i < m.nsensor; i++) {
+    int ds = intprm[3 * i], rd = intprm[3 * i + 1];
+    if ((ds & ~(1 | 2 | 8 | 16 | 32)) || (rd != 0 && rd != 3))
+      return fail("b2_create: contact sensor data/reduce combination not implemented");
+  }
+  return 0;
+}
 
-  // ---- derived integer tables ---------------------------------------------------------------
-  const std::vector<int>& parent = s->mi["body_parentid"];
-  const std::vector<int>& dofadr = s->mi["body_dofadr"];
-  const std::vector<int>& dofnum = s->mi["body_dofnum"];
+// Tables derived from the body tree: depths, ancestor chains, dof / ancestor / subtree masks, and the compact
+// kinematic records of the fast path (every body has at most one joint).
+static int kinematic_tables(b2_sim* s, const HostModel& h) {
+  DevModel& m = s->hm;
+  const std::vector<int>& parent = h.at(&DevModel::body_parentid);
+  const std::vector<int>& dofadr = h.at(&DevModel::body_dofadr);
+  const std::vector<int>& dofnum = h.at(&DevModel::body_dofnum);
   int nb = m.nbody;
   std::vector<int> depth(nb, 0);
   std::vector<unsigned long long> dofmask(nb, 0ull), ancmask(nb, 0ull);
@@ -477,327 +500,280 @@ int b2_create(const B2ModelDesc* desc, int nworld, int ncon_per_world, int njmax
   for (int b = 1; b < nb; b++)
     for (int i = 0; i < m.nv; i++)
       if (dofmask[b] >> i & 1ull) dofbody[i] |= 1ull << b;
-  // compact kinematic records (fast path: every body has at most one joint)
   std::vector<float> kinrec((size_t)nb * 16, 0.f);
   int fastkin = 1;
-  {
-    const std::vector<int>& jn = s->mi["body_jntnum"]; const std::vector<int>& ja = s->mi["body_jntadr"];
-    const std::vector<double>& bp = s->mf["body_pos"]; const std::vector<double>& bq = s->mf["body_quat"];
-    const std::vector<double>& jp = s->mf["jnt_pos"]; const std::vector<double>& jax = s->mf["jnt_axis"];
-    const std::vector<double>& q0 = s->mf["qpos0"];
-    for (int b = 0; b < nb; b++) {
-      if (jn[b] > 1) { fastkin = 0; break; }
-      float* r = kinrec.data() + 16 * b;
-      for (int k = 0; k < 3; k++) r[k] = (float)bp[3 * b + k];
-      for (int k = 0; k < 4; k++) r[4 + k] = (float)bq[4 * b + k];
-      int type = 0xff, j = 0, qa = 0;
-      if (jn[b] == 1) {
-        j = ja[b]; type = s->mi["jnt_type"][j]; qa = s->mi["jnt_qposadr"][j];
-        for (int k = 0; k < 3; k++) { r[8 + k] = (float)jp[3 * j + k]; r[12 + k] = (float)jax[3 * j + k]; }
-        r[3] = (float)q0[qa];
-      }
-      int tj = type | (j << 8);
-      memcpy(&r[11], &tj, 4);
-      memcpy(&r[15], &qa, 4);
+  const std::vector<int>& jn = h.at(&DevModel::body_jntnum); const std::vector<int>& ja = h.at(&DevModel::body_jntadr);
+  const std::vector<int>& jt = h.at(&DevModel::jnt_type); const std::vector<int>& jq = h.at(&DevModel::jnt_qposadr);
+  const std::vector<double>& bp = h.at(&DevModel::body_pos); const std::vector<double>& bq = h.at(&DevModel::body_quat);
+  const std::vector<double>& jp = h.at(&DevModel::jnt_pos); const std::vector<double>& jax = h.at(&DevModel::jnt_axis);
+  const std::vector<double>& q0 = h.at(&DevModel::qpos0);
+  for (int b = 0; b < nb; b++) {
+    if (jn[b] > 1) { fastkin = 0; break; }
+    float* r = kinrec.data() + 16 * b;
+    for (int k = 0; k < 3; k++) r[k] = (float)bp[3 * b + k];
+    for (int k = 0; k < 4; k++) r[4 + k] = (float)bq[4 * b + k];
+    int type = 0xff, j = 0, qa = 0;
+    if (jn[b] == 1) {
+      j = ja[b]; type = jt[j]; qa = jq[j];
+      for (int k = 0; k < 3; k++) { r[8 + k] = (float)jp[3 * j + k]; r[12 + k] = (float)jax[3 * j + k]; }
+      r[3] = (float)q0[qa];
     }
+    int tj = type | (j << 8);
+    memcpy(&r[11], &tj, 4);
+    memcpy(&r[15], &qa, 4);
   }
   m.fastkin = fastkin;
-  // World pose (pos[3], mat[9], rbound) of a geom on a jointless child of the world body, in double from world 0's
-  // model values: such geoms never move, so they are posed here once and shared by all worlds.
-  auto welded = [&](int g) { int b = s->mi["geom_bodyid"][g]; return b == 0 || (parent[b] == 0 && dofnum[b] == 0); };
-  auto world_pose = [&](int g, float* o) {
-    const std::vector<double>& bp = s->mf["body_pos"]; const std::vector<double>& bq = s->mf["body_quat"];
-    const std::vector<double>& gp = s->mf["geom_pos"]; const std::vector<double>& gq = s->mf["geom_quat"];
-    auto qmul = [](const double* a, const double* b, double* r) {
-      r[0] = a[0]*b[0] - a[1]*b[1] - a[2]*b[2] - a[3]*b[3];
-      r[1] = a[0]*b[1] + a[1]*b[0] + a[2]*b[3] - a[3]*b[2];
-      r[2] = a[0]*b[2] - a[1]*b[3] + a[2]*b[0] + a[3]*b[1];
-      r[3] = a[0]*b[3] + a[1]*b[2] - a[2]*b[1] + a[3]*b[0];
-    };
-    auto q2m = [](const double* q, double* R) {
-      R[0] = q[0]*q[0] + q[1]*q[1] - q[2]*q[2] - q[3]*q[3]; R[1] = 2*(q[1]*q[2] - q[0]*q[3]); R[2] = 2*(q[1]*q[3] + q[0]*q[2]);
-      R[3] = 2*(q[1]*q[2] + q[0]*q[3]); R[4] = q[0]*q[0] - q[1]*q[1] + q[2]*q[2] - q[3]*q[3]; R[5] = 2*(q[2]*q[3] - q[0]*q[1]);
-      R[6] = 2*(q[1]*q[3] - q[0]*q[2]); R[7] = 2*(q[2]*q[3] + q[0]*q[1]); R[8] = q[0]*q[0] - q[1]*q[1] - q[2]*q[2] + q[3]*q[3];
-    };
-    const int b = s->mi["geom_bodyid"][g];
-    double Rb[9], q[4], R[9];
-    q2m(&bq[4 * b], Rb);
-    qmul(&bq[4 * b], &gq[4 * g], q);
-    double nq = std::sqrt(q[0]*q[0] + q[1]*q[1] + q[2]*q[2] + q[3]*q[3]);
-    for (double& x : q) x /= nq;
-    q2m(q, R);
-    for (int i = 0; i < 3; i++)
-      o[i] = (float)(bp[3 * b + i] + Rb[3 * i] * gp[3 * g] + Rb[3 * i + 1] * gp[3 * g + 1] + Rb[3 * i + 2] * gp[3 * g + 2]);
-    for (int i = 0; i < 9; i++) o[3 + i] = (float)R[i];
-    o[12] = (float)s->mf["geom_rbound"][g];
+  const float* kr = nullptr;
+  int rc = dev_upload<int>(s, depth, &m.body_depth) || dev_upload<int>(s, chain, &m.body_chain) ||
+           dev_upload<unsigned long long>(s, dofmask, &m.body_dofmask) || dev_upload<unsigned long long>(s, ancmask, &m.body_ancmask) ||
+           dev_upload<unsigned long long>(s, submask, &m.body_submask) || dev_upload<unsigned long long>(s, dofbody, &m.dof_bodymask) ||
+           dev_upload<float>(s, kinrec, &kr);
+  m.kinrec = (const float4*)kr;
+  return rc;
+}
+
+// World pose (pos[3], mat[9], rbound) of a geom on a jointless child of the world body, in double from world 0's
+// model values: such geoms never move, so they are posed here once and shared by all worlds.
+static void world_pose(const HostModel& h, int g, float* o) {
+  const std::vector<double>& bp = h.at(&DevModel::body_pos); const std::vector<double>& bq = h.at(&DevModel::body_quat);
+  const std::vector<double>& gp = h.at(&DevModel::geom_pos); const std::vector<double>& gq = h.at(&DevModel::geom_quat);
+  auto qmul = [](const double* a, const double* b, double* r) {
+    r[0] = a[0]*b[0] - a[1]*b[1] - a[2]*b[2] - a[3]*b[3];
+    r[1] = a[0]*b[1] + a[1]*b[0] + a[2]*b[3] - a[3]*b[2];
+    r[2] = a[0]*b[2] - a[1]*b[3] + a[2]*b[0] + a[3]*b[1];
+    r[3] = a[0]*b[3] + a[1]*b[2] - a[2]*b[1] + a[3]*b[0];
   };
-  // Pose slots of the collision geoms in shared memory.  Height fields welded to the world (a terrain has tens of
-  // them) get no slot: their pose records live in global memory (fixed_pose, slot code -2 - index) - 56 bytes of
-  // shared memory per field and per environment otherwise, and a pose computation per step.
-  std::vector<int> cslot(m.ngeom, -1), cgeom, fixed_geom;
+  auto q2m = [](const double* q, double* R) {
+    R[0] = q[0]*q[0] + q[1]*q[1] - q[2]*q[2] - q[3]*q[3]; R[1] = 2*(q[1]*q[2] - q[0]*q[3]); R[2] = 2*(q[1]*q[3] + q[0]*q[2]);
+    R[3] = 2*(q[1]*q[2] + q[0]*q[3]); R[4] = q[0]*q[0] - q[1]*q[1] + q[2]*q[2] - q[3]*q[3]; R[5] = 2*(q[2]*q[3] - q[0]*q[1]);
+    R[6] = 2*(q[1]*q[3] - q[0]*q[2]); R[7] = 2*(q[2]*q[3] + q[0]*q[1]); R[8] = q[0]*q[0] - q[1]*q[1] - q[2]*q[2] + q[3]*q[3];
+  };
+  const int b = h.at(&DevModel::geom_bodyid)[g];
+  double Rb[9], q[4], R[9];
+  q2m(&bq[4 * b], Rb);
+  qmul(&bq[4 * b], &gq[4 * g], q);
+  double nq = std::sqrt(q[0]*q[0] + q[1]*q[1] + q[2]*q[2] + q[3]*q[3]);
+  for (double& x : q) x /= nq;
+  q2m(q, R);
+  for (int i = 0; i < 3; i++)
+    o[i] = (float)(bp[3 * b + i] + Rb[3 * i] * gp[3 * g] + Rb[3 * i + 1] * gp[3 * g + 1] + Rb[3 * i + 2] * gp[3 * g + 2]);
+  for (int i = 0; i < 9; i++) o[3 + i] = (float)R[i];
+  o[12] = (float)h.at(&DevModel::geom_rbound)[g];
+}
+
+// Collision plan: pose slots of the collision geoms, the grid-static set, a narrowphase routine for every pair, the
+// broadphase pair words and the height-field pairs grouped by field.
+static int collision_plan(b2_sim* s, const HostModel& h) {
+  DevModel& m = s->hm;
+  const std::vector<int>& parent = h.at(&DevModel::body_parentid); const std::vector<int>& dofnum = h.at(&DevModel::body_dofnum);
+  const std::vector<int>& bodyid = h.at(&DevModel::geom_bodyid); const std::vector<int>& gt = h.at(&DevModel::geom_type);
+  const std::vector<int>& pg1 = h.at(&DevModel::pair_geom1); const std::vector<int>& pg2 = h.at(&DevModel::pair_geom2);
+  const std::vector<int>& sg = h.at(&DevModel::static_geom); const std::vector<int>& dyn = h.at(&DevModel::dyn_cgeom);
+  const std::vector<int>& did = h.at(&DevModel::geom_dataid);
+  std::vector<int> cslot(m.ngeom, -1), cgeom, fixed_geom, posegeom;  // (cslot: pose slot, or -2 - index into fixed_pose)
+  auto welded = [&](int g) { int b = bodyid[g]; return b == 0 || (parent[b] == 0 && dofnum[b] == 0); };
+  // Height fields welded to the world (a terrain has tens of them) get no slot: their pose records live in global
+  // memory (fixed_pose, slot code -2 - index) - 56 bytes of shared memory per field and per environment otherwise,
+  // and a pose computation per step.
   {
     std::vector<char> second(m.ngeom, 0);
-    for (int p = 0; p < m.npair; p++) second[s->mi["pair_geom2"][p]] = 1;
+    for (int p = 0; p < m.npair; p++) second[pg2[p]] = 1;
     for (int p = 0; p < m.npair; p++) {
-      for (int g : {s->mi["pair_geom1"][p], s->mi["pair_geom2"][p]}) {
+      for (int g : {pg1[p], pg2[p]}) {
         if (cslot[g] != -1) continue;
-        if (s->mi["geom_type"][g] == G_HFIELD && !second[g] && welded(g)) { cslot[g] = -2 - (int)fixed_geom.size(); fixed_geom.push_back(g); }
+        if (gt[g] == G_HFIELD && !second[g] && welded(g)) { cslot[g] = -2 - (int)fixed_geom.size(); fixed_geom.push_back(g); }
         else { cslot[g] = (int)cgeom.size(); cgeom.push_back(g); }
       }
     }
   }
   m.nfixed = (int)fixed_geom.size();
   std::vector<float> fixed_pose((size_t)std::max(m.nfixed, 1) * 16, 0.f);
-  for (int f = 0; f < m.nfixed; f++) world_pose(fixed_geom[f], fixed_pose.data() + 16 * (size_t)f);
+  for (int f = 0; f < m.nfixed; f++) world_pose(h, fixed_geom[f], fixed_pose.data() + 16 * (size_t)f);
   // grid-static collision set: static geoms never move, so their world poses are computed here once (in
   // double, from world 0's model values) and shared by all worlds; only the other geoms are posed per step
-  m.nstatic = geti("nstatic");
-  m.ndyn = (int)s->mi["dyn_cgeom"].size();
-  std::vector<int> posegeom;
+  m.nstatic = (int)h.scalar("nstatic");
+  m.ndyn = (int)dyn.size();
   std::vector<float> static_pose((size_t)std::max(m.nstatic, 1) * 16, 0.f);
-  {
-    std::vector<char> is_static(m.ngeom, 0);
-    const std::vector<int>& sg = s->mi["static_geom"];
-    if ((int)sg.size() != m.nstatic) { delete s; return fail("b2_create: static_geom / nstatic mismatch"); }
-    if (m.nstatic >= (1 << 20) || m.ndyn >= (1 << 11)) { delete s; return fail("b2_create: static grid too large"); }
-    for (int k = 0; k < m.nstatic; k++) {
-      int g = sg[k], b = s->mi["geom_bodyid"][g];
-      if (g < 0 || g >= m.ngeom || parent[b] != 0 || dofnum[b] != 0) {
-        delete s;
-        return fail("b2_create: grid-static geoms must sit on a jointless child of the world body");
-      }
-      is_static[g] = 1;
-      world_pose(g, static_pose.data() + 16 * (size_t)k);
-    }
-    for (int g : fixed_geom) is_static[g] = 1;
-    for (int g = 0; g < m.ngeom; g++) if (!is_static[g]) posegeom.push_back(g);
-    m.nposegeom = (int)posegeom.size();
-    for (int g : s->mi["dyn_cgeom"]) {
-      if (g < 0 || g >= m.ngeom || is_static[g]) { delete s; return fail("b2_create: bad dyn_cgeom entry"); }
-      if (cslot[g] < 0) { cslot[g] = (int)cgeom.size(); cgeom.push_back(g); }
-    }
-    if (m.nstatic > 0) {
-      const std::vector<double>& gpar = s->mf["grid_params"];
-      if (gpar.size() != 5) { delete s; return fail("b2_create: grid_params must hold [x0, y0, cell, nx, ny]"); }
-      m.grid_x0 = (float)gpar[0]; m.grid_y0 = (float)gpar[1]; m.grid_cell = (float)gpar[2];
-      m.grid_nx = (int)gpar[3]; m.grid_ny = (int)gpar[4];
-      if ((int)s->mi["grid_start"].size() != m.grid_nx * m.grid_ny + 1 || (int)s->mi["static_cell0"].size() != 2 * m.nstatic) {
-        delete s;
-        return fail("b2_create: static grid tables have inconsistent sizes");
-      }
-    }
+  std::vector<char> is_static(m.ngeom, 0);
+  if ((int)sg.size() != m.nstatic) return fail("b2_create: static_geom / nstatic mismatch");
+  if (m.nstatic >= (1 << 20) || m.ndyn >= (1 << 11)) return fail("b2_create: static grid too large");
+  for (int k = 0; k < m.nstatic; k++) {
+    int g = sg[k], b = bodyid[g];
+    if (g < 0 || g >= m.ngeom || parent[b] != 0 || dofnum[b] != 0)
+      return fail("b2_create: grid-static geoms must sit on a jointless child of the world body");
+    is_static[g] = 1;
+    world_pose(h, g, static_pose.data() + 16 * (size_t)k);
+  }
+  for (int g : fixed_geom) is_static[g] = 1;
+  for (int g = 0; g < m.ngeom; g++) if (!is_static[g]) posegeom.push_back(g);
+  m.nposegeom = (int)posegeom.size();
+  for (int g : dyn) {
+    if (g < 0 || g >= m.ngeom || is_static[g]) return fail("b2_create: bad dyn_cgeom entry");
+    if (cslot[g] < 0) { cslot[g] = (int)cgeom.size(); cgeom.push_back(g); }
+  }
+  if (m.nstatic > 0) {
+    const std::vector<double>& gpar = HostModel::find(h.f, "grid_params");
+    if (gpar.size() != 5) return fail("b2_create: grid_params must hold [x0, y0, cell, nx, ny]");
+    m.grid_x0 = (float)gpar[0]; m.grid_y0 = (float)gpar[1]; m.grid_cell = (float)gpar[2];
+    m.grid_nx = (int)gpar[3]; m.grid_ny = (int)gpar[4];
+    if ((int)h.at(&DevModel::grid_start).size() != m.grid_nx * m.grid_ny + 1 || (int)h.at(&DevModel::static_cell0).size() != 2 * m.nstatic)
+      return fail("b2_create: static grid tables have inconsistent sizes");
   }
   m.ncg = (int)cgeom.size();
-  {  // every collision pair must have a narrowphase routine (primitives, or the convex routines of b2_convex.h)
-    const std::vector<int>& gt = s->mi["geom_type"];
-    auto prim = [](int t) { return t == G_SPHERE || t == G_CAPSULE || t == G_BOX; };
-    auto smooth = [](int t) { return t == G_ELLIPSOID || t == G_CYLINDER; };
-    auto conv = [&](int t) { return prim(t) || t == G_MESH || smooth(t); };  // shapes the GJK/EPA routine takes (b2_convex.h)
-    const std::vector<int>& did = s->mi["geom_dataid"];
-    const int nmesh = (int)s->mi["mesh_vertnum"].size(), nhf = (int)s->mi["hfield_nrow"].size();
-    for (int p = 0; p < m.npair; p++) {
-      int g1 = s->mi["pair_geom1"][p], g2 = s->mi["pair_geom2"][p];
-      int t1 = gt[g1], t2 = gt[g2];
-      bool ok = (t1 == G_PLANE && conv(t2)) || (t1 == G_HFIELD && conv(t2)) || (conv(t1) && conv(t2) && t1 <= t2);
-      if (t2 == G_MESH || t1 == G_HFIELD || smooth(t1) || smooth(t2)) s->has_convex = 1;
-      if (!ok) { delete s; return fail("b2_create: collision pair with an unsupported geom type combination"); }
-      for (int g : {g1, g2}) {
-        int t = gt[g];
-        if (t != G_MESH && t != G_HFIELD) continue;
-        int id = g < (int)did.size() ? did[g] : -1;
-        if (id < 0 || id >= (t == G_MESH ? nmesh : nhf)) { delete s; return fail("b2_create: colliding mesh / hfield geom without asset data (geom_dataid)"); }
-        if (t == G_MESH && (s->mi["mesh_vertnum"][id] < 1 || (size_t)3 * (s->mi["mesh_vertadr"][id] + s->mi["mesh_vertnum"][id]) > s->mf["mesh_vert"].size())) {
-          delete s; return fail("b2_create: mesh vertex range outside mesh_vert");
-        }
-        if (t == G_HFIELD && (s->mi["hfield_nrow"][id] < 2 || s->mi["hfield_ncol"][id] < 2 || (size_t)4 * (id + 1) > s->mf["hfield_size"].size() ||
-                              (size_t)s->mi["hfield_adr"][id] + (size_t)s->mi["hfield_nrow"][id] * s->mi["hfield_ncol"][id] > s->mf["hfield_data"].size())) {
-          delete s; return fail("b2_create: hfield sample range outside hfield_data");
-        }
-      }
+  // every collision pair must have a narrowphase routine (primitives, or the convex routines of b2_convex.h)
+  auto prim = [](int t) { return t == G_SPHERE || t == G_CAPSULE || t == G_BOX; };
+  auto smooth = [](int t) { return t == G_ELLIPSOID || t == G_CYLINDER; };
+  auto conv = [&](int t) { return prim(t) || t == G_MESH || smooth(t); };  // shapes the GJK/EPA routine takes (b2_convex.h)
+  const std::vector<int>& vadr = h.at(&DevModel::mesh_vertadr); const std::vector<int>& vnum = h.at(&DevModel::mesh_vertnum);
+  const std::vector<int>& hadr = h.at(&DevModel::hfield_adr); const std::vector<int>& hrow = h.at(&DevModel::hfield_nrow);
+  const std::vector<int>& hcol = h.at(&DevModel::hfield_ncol); const std::vector<double>& hsize = h.at(&DevModel::hfield_size);
+  const size_t nvert = h.at(&DevModel::mesh_vert).size(), nhdata = h.at(&DevModel::hfield_data).size();
+  const int nmesh = (int)vnum.size(), nhf = (int)hrow.size();
+  for (int p = 0; p < m.npair; p++) {
+    int g1 = pg1[p], g2 = pg2[p];
+    int t1 = gt[g1], t2 = gt[g2];
+    bool ok = (t1 == G_PLANE && conv(t2)) || (t1 == G_HFIELD && conv(t2)) || (conv(t1) && conv(t2) && t1 <= t2);
+    if (t2 == G_MESH || t1 == G_HFIELD || smooth(t1) || smooth(t2)) s->has_convex = 1;
+    if (!ok) return fail("b2_create: collision pair with an unsupported geom type combination");
+    for (int g : {g1, g2}) {
+      int t = gt[g];
+      if (t != G_MESH && t != G_HFIELD) continue;
+      int id = g < (int)did.size() ? did[g] : -1;
+      if (id < 0 || id >= (t == G_MESH ? nmesh : nhf)) return fail("b2_create: colliding mesh / hfield geom without asset data (geom_dataid)");
+      if (t == G_MESH && (vnum[id] < 1 || (size_t)3 * (vadr[id] + vnum[id]) > nvert))
+        return fail("b2_create: mesh vertex range outside mesh_vert");
+      if (t == G_HFIELD && (hrow[id] < 2 || hcol[id] < 2 || (size_t)4 * (id + 1) > hsize.size() ||
+                            (size_t)hadr[id] + (size_t)hrow[id] * hcol[id] > nhdata))
+        return fail("b2_create: hfield sample range outside hfield_data");
     }
-    for (int g : s->mi["dyn_cgeom"]) {
-      if (!conv(gt[g])) { delete s; return fail("b2_create: unsupported dynamic geom type for the static grid"); }
-      if (gt[g] == G_MESH || smooth(gt[g])) s->has_convex = 1;
-    }
-    for (int g : s->mi["static_geom"]) if (!prim(gt[g])) { delete s; return fail("b2_create: unsupported grid-static geom type"); }
   }
+  for (int g : dyn) {
+    if (!conv(gt[g])) return fail("b2_create: unsupported dynamic geom type for the static grid");
+    if (gt[g] == G_MESH || smooth(gt[g])) s->has_convex = 1;
+  }
+  for (int g : sg) if (!prim(gt[g])) return fail("b2_create: unsupported grid-static geom type");
+  if (m.ncg >= 4096) return fail("b2_create: too many collision geoms");
   int rc = 0;
-#define UPI(field, key) rc |= dev_upload<int>(s, s->mi[key], &m.field)
-  UPI(body_parentid, "body_parentid"); UPI(body_rootid, "body_rootid"); UPI(body_jntadr, "body_jntadr");
-  UPI(body_jntnum, "body_jntnum"); UPI(body_dofadr, "body_dofadr"); UPI(body_dofnum, "body_dofnum");
-  UPI(jnt_type, "jnt_type"); UPI(jnt_qposadr, "jnt_qposadr"); UPI(jnt_dofadr, "jnt_dofadr");
-  UPI(jnt_bodyid, "jnt_bodyid"); UPI(jnt_limited, "jnt_limited"); UPI(dof_bodyid, "dof_bodyid");
-  UPI(dof_jntid, "dof_jntid"); UPI(dof_parentid, "dof_parentid"); UPI(geom_type, "geom_type");
-  UPI(geom_bodyid, "geom_bodyid"); UPI(geom_condim, "geom_condim"); UPI(geom_priority, "geom_priority");
-  UPI(site_bodyid, "site_bodyid"); UPI(actuator_trnid, "actuator_trnid");
-  UPI(actuator_ctrllimited, "actuator_ctrllimited"); UPI(actuator_forcelimited, "actuator_forcelimited");
-  UPI(pair_geom1, "pair_geom1"); UPI(pair_geom2, "pair_geom2"); UPI(sensor_objtype, "sensor_objtype");
-  UPI(geom_contype, "geom_contype"); UPI(geom_conaffinity, "geom_conaffinity"); UPI(dyn_cgeom, "dyn_cgeom");
-  UPI(static_geom, "static_geom"); UPI(static_cell0, "static_cell0"); UPI(grid_start, "grid_start");
-  UPI(grid_items, "grid_items");
-  UPI(geom_dataid, "geom_dataid"); UPI(mesh_vertadr, "mesh_vertadr"); UPI(mesh_vertnum, "mesh_vertnum");
-  UPI(hfield_adr, "hfield_adr"); UPI(hfield_nrow, "hfield_nrow"); UPI(hfield_ncol, "hfield_ncol");
-  UPI(sensor_objid, "sensor_objid"); UPI(sensor_reftype, "sensor_reftype");
-  UPI(sensor_refid, "sensor_refid"); UPI(sensor_intprm, "sensor_intprm"); UPI(sensor_adr, "sensor_adr");
-  UPI(sensor_dim, "sensor_dim");
-#undef UPI
-  rc |= dev_upload<int>(s, depth, &m.body_depth);
-  rc |= dev_upload<int>(s, chain, &m.body_chain);
-  rc |= dev_upload<unsigned long long>(s, dofmask, &m.body_dofmask);
-  rc |= dev_upload<unsigned long long>(s, ancmask, &m.body_ancmask);
-  rc |= dev_upload<unsigned long long>(s, submask, &m.body_submask);
-  rc |= dev_upload<unsigned long long>(s, dofbody, &m.dof_bodymask);
-  {
-    const float* kr = nullptr;
-    rc |= dev_upload<float>(s, kinrec, &kr);
-    m.kinrec = (const float4*)kr;
+  std::vector<unsigned> pw(std::max(m.npair, 1), 0u);
+  for (int p = 0; p < m.npair; p++) {
+    int g1 = pg1[p], g2 = pg2[p];
+    pw[p] = (unsigned)std::max(cslot[g1], 0) | ((unsigned)std::max(cslot[g2], 0) << 12) | (gt[g1] == G_PLANE ? 0x80000000u : 0u) |
+            (gt[g1] == G_HFIELD ? 0x40000000u : 0u);
   }
-  for (auto kv : {std::make_pair("mesh_vert", &m.mesh_vert), std::make_pair("hfield_size", &m.hfield_size),
-                  std::make_pair("hfield_data", &m.hfield_data)}) {
-    const std::vector<double>& h = s->mf[kv.first];
-    std::vector<float> hf(h.begin(), h.end());
-    rc |= dev_upload<float>(s, hf, kv.second);
+  rc |= dev_upload<unsigned>(s, pw, &m.pair_word);
+  // height-field pairs grouped by field: the kernel first finds the fields under the robot, then tests only
+  // their pairs (a terrain is a grid of fields; the flat pair table would test every one of them)
+  std::vector<int> hf_geom, hf_slot, hf_start, hf_pairs, hfd, nh;  // (hf_slot: pose slot, or -2 - index into fixed_pose)
+  std::vector<std::vector<int>> per;
+  std::vector<float> box;
+  for (int p = 0; p < m.npair; p++) {
+    int g1 = pg1[p], g2 = pg2[p];
+    if (gt[g1] != G_HFIELD) { nh.push_back(p); continue; }
+    size_t k = std::find(hf_geom.begin(), hf_geom.end(), g1) - hf_geom.begin();
+    if (k == hf_geom.size()) {
+      hf_geom.push_back(g1); hf_slot.push_back(cslot[g1]); per.emplace_back();
+      for (int j = 0; j < 4; j++) box.push_back((float)hsize[4 * (size_t)did[g1] + j]);
+    }
+    per[k].push_back(p);
+    if (std::find(hfd.begin(), hfd.end(), cslot[g2]) == hfd.end()) hfd.push_back(cslot[g2]);
+  }
+  m.nhf = (int)hf_geom.size(); m.nhfd = (int)hfd.size(); m.n_nhpair = m.npair;
+  m.hfl_slot = m.hfl_geom = m.hfl_start = m.hfl_pairs = m.hfd_slot = m.nh_pairs = nullptr; m.hfl_box = nullptr;
+  if (m.nhf > 0) {
+    for (auto& v : per) { hf_start.push_back((int)hf_pairs.size()); hf_pairs.insert(hf_pairs.end(), v.begin(), v.end()); }
+    hf_start.push_back((int)hf_pairs.size());
+    m.n_nhpair = (int)nh.size();
+    if (nh.empty()) nh.push_back(0);
+    const float* bp = nullptr;
+    rc |= dev_upload<int>(s, hf_slot, &m.hfl_slot); rc |= dev_upload<int>(s, hf_start, &m.hfl_start);
+    rc |= dev_upload<int>(s, hf_geom, &m.hfl_geom);
+    rc |= dev_upload<int>(s, hf_pairs, &m.hfl_pairs); rc |= dev_upload<int>(s, hfd, &m.hfd_slot);
+    rc |= dev_upload<int>(s, nh, &m.nh_pairs); rc |= dev_upload<float>(s, box, &bp);
+    m.hfl_box = (const float4*)bp;
   }
   rc |= dev_upload<int>(s, posegeom, &m.posegeom);
   rc |= dev_upload<float>(s, static_pose, &m.static_pose);
-  {
-    if (m.ncg >= 4096) { b2_destroy(s); return fail("b2_create: too many collision geoms"); }
-    std::vector<unsigned> pw(std::max(m.npair, 1), 0u);
-    for (int p = 0; p < m.npair; p++) {
-      int g1 = s->mi["pair_geom1"][p], g2 = s->mi["pair_geom2"][p];
-      pw[p] = (unsigned)std::max(cslot[g1], 0) | ((unsigned)std::max(cslot[g2], 0) << 12) | (s->mi["geom_type"][g1] == G_PLANE ? 0x80000000u : 0u) |
-              (s->mi["geom_type"][g1] == G_HFIELD ? 0x40000000u : 0u);
-    }
-    rc |= dev_upload<unsigned>(s, pw, &m.pair_word);
-    // height-field pairs grouped by field: the kernel first finds the fields under the robot, then tests only
-    // their pairs (a terrain is a grid of fields; the flat pair table would test every one of them)
-    std::vector<int> hf_geom, hf_slot, hf_start, hf_pairs, hfd, nh;  // (hf_slot: pose slot, or -2 - index into fixed_pose)
-    std::vector<std::vector<int>> per;
-    std::vector<float> box;
-    for (int p = 0; p < m.npair; p++) {
-      int g1 = s->mi["pair_geom1"][p], g2 = s->mi["pair_geom2"][p];
-      if (s->mi["geom_type"][g1] != G_HFIELD) { nh.push_back(p); continue; }
-      size_t h = std::find(hf_geom.begin(), hf_geom.end(), g1) - hf_geom.begin();
-      if (h == hf_geom.size()) {
-        hf_geom.push_back(g1); hf_slot.push_back(cslot[g1]); per.emplace_back();
-        const int id = s->mi["geom_dataid"][g1];
-        for (int k = 0; k < 4; k++) box.push_back((float)s->mf["hfield_size"][4 * (size_t)id + k]);
-      }
-      per[h].push_back(p);
-      if (std::find(hfd.begin(), hfd.end(), cslot[g2]) == hfd.end()) hfd.push_back(cslot[g2]);
-    }
-    m.nhf = (int)hf_geom.size(); m.nhfd = (int)hfd.size(); m.n_nhpair = m.npair;
-    m.hfl_slot = m.hfl_geom = m.hfl_start = m.hfl_pairs = m.hfd_slot = m.nh_pairs = nullptr; m.hfl_box = nullptr;
-    if (m.nhf > 0) {
-      for (auto& v : per) { hf_start.push_back((int)hf_pairs.size()); hf_pairs.insert(hf_pairs.end(), v.begin(), v.end()); }
-      hf_start.push_back((int)hf_pairs.size());
-      m.n_nhpair = (int)nh.size();
-      if (nh.empty()) nh.push_back(0);
-      const float* bp = nullptr;
-      rc |= dev_upload<int>(s, hf_slot, &m.hfl_slot); rc |= dev_upload<int>(s, hf_start, &m.hfl_start);
-      rc |= dev_upload<int>(s, hf_geom, &m.hfl_geom);
-      rc |= dev_upload<int>(s, hf_pairs, &m.hfl_pairs); rc |= dev_upload<int>(s, hfd, &m.hfd_slot);
-      rc |= dev_upload<int>(s, nh, &m.nh_pairs); rc |= dev_upload<float>(s, box, &bp);
-      m.hfl_box = (const float4*)bp;
-    }
-  }
   rc |= dev_upload<int>(s, cslot, &m.geom_cslot);
   rc |= dev_upload<float>(s, fixed_pose, &m.fixed_pose);
   if (fixed_geom.empty()) fixed_geom.push_back(0);
   rc |= dev_upload<int>(s, fixed_geom, &m.fixed_geom);
   rc |= dev_upload<int>(s, cgeom, &m.cgeom);
-  {
-    // schedules of the bottom-up blocked factorisation (b2_kernel.cuh: ldl_factor)
-    std::vector<unsigned> dense, sparse;
-    b2_build_ldl_schedules(m.nv, s->mi["dof_parentid"].data(), dense, sparse, m.ldl_start);
-    m.ldl_nsparse = (int)sparse.size();
-    rc |= dev_upload<unsigned>(s, dense, &m.ldl_dense);
-    rc |= dev_upload<unsigned>(s, sparse, &m.ldl_sparse);
-  }
-  if (rc) { b2_destroy(s); return 1; }
-  // supported sensor set: contact sensors with data in {found,force,dist,pos,normal}, reduce none/netforce
-  for (int i = 0; i < m.nsensor; i++) {
-    int ds = s->mi["sensor_intprm"][3 * i], rd = s->mi["sensor_intprm"][3 * i + 1];
-    if ((ds & ~(1 | 2 | 8 | 16 | 32)) || (rd != 0 && rd != 3)) {
-      b2_destroy(s);
-      return fail("b2_create: contact sensor data/reduce combination not implemented");
+  return rc;
+}
+
+// The model's arrays on the device (fp32 floats, shared by all worlds), its Model fields, and the schedules of the
+// bottom-up blocked factorisation (b2_kernel.cuh: ldl_factor).
+static int upload_model(b2_sim* s, const HostModel& h) {
+  DevModel& m = s->hm;
+  for (const IntArray& r : kIntArrays) {
+    if (dev_upload<int>(s, h.at(r.dev), &(m.*r.dev))) return 1;
+    if (r.field) {  // 1-D, shared by all worlds
+      Field f; f.name = r.name; f.ptr = (void*)(m.*r.dev); f.dtype = B2_I32; f.ndim = 1;
+      f.n = f.shape[0] = (int64_t)h.at(r.dev).size(); f.stride[0] = 1;
+      s->model_fields.push_back(f);
     }
   }
-  // int model fields visible to callers
-  auto add_imodel = [&](const char* name, const int* p, int n) {
-    Field f; f.name = name; f.ptr = (void*)p; f.dtype = B2_I32; f.ndim = 1; f.shape[0] = n; f.stride[0] = 1; f.n = n;
-    s->model_fields.push_back(f);
-  };
-  add_imodel("geom_bodyid", m.geom_bodyid, m.ngeom); add_imodel("site_bodyid", m.site_bodyid, m.nsite);
-  add_imodel("body_parentid", m.body_parentid, nb); add_imodel("body_rootid", m.body_rootid, nb);
-  add_imodel("jnt_type", m.jnt_type, m.njnt); add_imodel("jnt_qposadr", m.jnt_qposadr, m.njnt);
-  add_imodel("jnt_dofadr", m.jnt_dofadr, m.njnt); add_imodel("dof_bodyid", m.dof_bodyid, m.nv);
-  add_imodel("geom_type", m.geom_type, m.ngeom); add_imodel("geom_condim", m.geom_condim, m.ngeom);
-  add_imodel("geom_priority", m.geom_priority, m.ngeom);
-  add_imodel("actuator_trnid", m.actuator_trnid, m.nu);
-
-  // ---- float model arrays (fp32 on device; shared by all worlds until expanded) -----------------
-  for (const ShapeSpec& sp : kModelShapes) {
-    const std::vector<double>& h = s->mf[sp.name];
-    std::vector<float> hf(h.begin(), h.end());
+  for (const AssetArray& r : kAssetArrays) {
+    const std::vector<double>& v = h.at(r.dev);
+    if (dev_upload<float>(s, std::vector<float>(v.begin(), v.end()), &(m.*r.dev))) return 1;
+  }
+  for (const FloatArray& r : kFloatArrays) {
+    const std::vector<double>& v = h.at(r.dev);
     const float* p = nullptr;
-    if (dev_upload<float>(s, hf, &p)) { b2_destroy(s); return 1; }
-    FArr* fa = model_farr(m, sp.name);
-    fa->p = p; fa->stride = 0; fa->n = (int)hf.size();
-    Field f; f.name = sp.name; f.ptr = (void*)p; f.dtype = B2_F32; f.farr = fa; f.n = (int64_t)hf.size();
-    if (sp.second > 0) {
-      f.ndim = 3; f.shape[0] = nworld; f.shape[1] = (int64_t)hf.size() / sp.second; f.shape[2] = sp.second;
-      f.stride[0] = 0; f.stride[1] = sp.second; f.stride[2] = 1;
-    } else {
-      f.ndim = 2; f.shape[0] = nworld; f.shape[1] = (int64_t)hf.size(); f.stride[0] = 0; f.stride[1] = 1;
-    }
+    if (dev_upload<float>(s, std::vector<float>(v.begin(), v.end()), &p)) return 1;
+    FArr& fa = m.*r.dev;
+    fa.p = p; fa.stride = 0; fa.n = (int)v.size();
+    Field f = make_field(r.name, (void*)p, B2_F32, s->nworld, 0, (int64_t)v.size(), r.width, false);
+    f.farr = &fa;
     s->model_fields.push_back(f);
   }
+  std::vector<unsigned> dense, sparse;
+  b2_build_ldl_schedules(m.nv, h.at(&DevModel::dof_parentid).data(), dense, sparse, m.ldl_start);
+  m.ldl_nsparse = (int)sparse.size();
+  return dev_upload<unsigned>(s, dense, &m.ldl_dense) || dev_upload<unsigned>(s, sparse, &m.ldl_sparse);
+}
 
-  // ---- data -------------------------------------------------------------------------------------
+// Per-world Data arrays (zeroed), registered as Data fields in this order.
+static int alloc_data(b2_sim* s) {
+  const DevModel& m = s->hm;
   DevData& d = s->hd;
   memset(&d, 0, sizeof(d));
-  d.nworld = nworld;
-  int nq = m.nq, nv = m.nv, nu = m.nu, ng = m.ngeom, ns = m.nsite, mc = m.maxcon;
-  rc = 0;
-  rc |= add_data(s, "qpos", &d.qpos, nq); rc |= add_data(s, "qvel", &d.qvel, nv);
-  rc |= add_data(s, "ctrl", &d.ctrl, nu); rc |= add_data(s, "qacc_warmstart", &d.qacc_warmstart, nv);
-  rc |= add_data(s, "qfrc_applied", &d.qfrc_applied, nv);
-  rc |= add_data(s, "xfrc_applied", &d.xfrc_applied, 6 * nb, 6);
-  rc |= add_data(s, "act", &d.act, 0);
-  rc |= add_data(s, "qacc", &d.qacc, nv); rc |= add_data(s, "xpos", &d.xpos, 3 * nb, 3);
-  rc |= add_data(s, "xquat", &d.xquat, 4 * nb, 4); rc |= add_data(s, "xmat", &d.xmat, 9 * nb, 9);
-  rc |= add_data(s, "xipos", &d.xipos, 3 * nb, 3); rc |= add_data(s, "subtree_com", &d.subtree_com, 3 * nb, 3);
-  rc |= add_data(s, "cvel", &d.cvel, 6 * nb, 6); rc |= add_data(s, "geom_xpos", &d.geom_xpos, 3 * ng, 3);
-  rc |= add_data(s, "geom_xmat", &d.geom_xmat, 9 * ng, 9); rc |= add_data(s, "site_xpos", &d.site_xpos, 3 * ns, 3);
-  rc |= add_data(s, "site_xmat", &d.site_xmat, 9 * ns, 9);
-  rc |= add_data(s, "link_vel_w", &d.link_vel_w, 6 * nb, 6); rc |= add_data(s, "com_vel_w", &d.com_vel_w, 6 * nb, 6);
-  rc |= add_data(s, "link_state_b", &d.link_state_b, 10 * nb, 10);
-  rc |= add_data(s, "sensordata", &d.sensordata, m.nsensordata);
-  rc |= add_data(s, "actuator_force", &d.actuator_force, nu); rc |= add_data(s, "time", &d.time, 1);
-  rc |= add_data(s, "qfrc_bias", &d.qfrc_bias, nv); rc |= add_data(s, "qfrc_smooth", &d.qfrc_smooth, nv);
-  rc |= add_data(s, "qacc_smooth", &d.qacc_smooth, nv);
-  rc |= add_data(s, "qfrc_constraint", &d.qfrc_constraint, nv);
-  rc |= add_data(s, "qM", &d.qM, nv * nv, nv);
-  rc |= add_data(s, "qM_packed", &d.qM_packed, m.ntri);
-  rc |= add_data(s, "qacc_smooth_prev", &d.qacc_smooth_prev, nv);
-  rc |= add_data(s, "ctrl_prev", &d.ctrl_prev, nu);
-  rc |= add_data(s, "contact_dist", &d.contact_dist, mc); rc |= add_data(s, "contact_pos", &d.contact_pos, 3 * mc, 3);
-  rc |= add_data(s, "contact_frame", &d.contact_frame, 9 * mc, 9);
-  rc |= add_data(s, "contact_force", &d.contact_force, 3 * mc, 3);
-  rc |= add_data(s, "solver_cost", &d.solver_cost, 1);
-  rc |= add_idata(s, "ncon", &d.ncon, 1); rc |= add_idata(s, "nefc", &d.nefc, 1);
-  rc |= add_idata(s, "solver_niter", &d.solver_niter, 1);
-  rc |= add_idata(s, "contact_geom", &d.contact_geom, 2 * mc, 2);
-  rc |= add_idata(s, "overflow", &d.overflow, 1);
-  rc |= add_idata(s, "solver_nd", &d.solver_nd, 1);
-  rc |= add_idata(s, "solver_nls", &d.solver_nls, 1);  // line-search derivative evaluations of the last step (diagnostic)
-  if (rc) { b2_destroy(s); return 1; }
-  // time is exposed as a 1-D (nworld,) tensor
-  for (Field& f : s->data_fields)
-    if (f.name == "time" || f.name == "solver_cost") { f.ndim = 1; }
+  d.nworld = s->nworld;
+  const int nq = m.nq, nv = m.nv, nu = m.nu, nb = m.nbody, ng = m.ngeom, ns = m.nsite, mc = m.maxcon;
+  const DataArray<DArr> floats[] = {
+      {"qpos", &DevData::qpos, nq}, {"qvel", &DevData::qvel, nv}, {"ctrl", &DevData::ctrl, nu},
+      {"qacc_warmstart", &DevData::qacc_warmstart, nv}, {"qfrc_applied", &DevData::qfrc_applied, nv},
+      {"xfrc_applied", &DevData::xfrc_applied, 6 * nb, 6}, {"act", &DevData::act, 0}, {"qacc", &DevData::qacc, nv},
+      {"xpos", &DevData::xpos, 3 * nb, 3}, {"xquat", &DevData::xquat, 4 * nb, 4}, {"xmat", &DevData::xmat, 9 * nb, 9},
+      {"xipos", &DevData::xipos, 3 * nb, 3}, {"subtree_com", &DevData::subtree_com, 3 * nb, 3},
+      {"cvel", &DevData::cvel, 6 * nb, 6}, {"geom_xpos", &DevData::geom_xpos, 3 * ng, 3},
+      {"geom_xmat", &DevData::geom_xmat, 9 * ng, 9}, {"site_xpos", &DevData::site_xpos, 3 * ns, 3},
+      {"site_xmat", &DevData::site_xmat, 9 * ns, 9}, {"link_vel_w", &DevData::link_vel_w, 6 * nb, 6},
+      {"com_vel_w", &DevData::com_vel_w, 6 * nb, 6}, {"link_state_b", &DevData::link_state_b, 10 * nb, 10},
+      {"sensordata", &DevData::sensordata, m.nsensordata}, {"actuator_force", &DevData::actuator_force, nu},
+      {"time", &DevData::time, 1, 0, true}, {"qfrc_bias", &DevData::qfrc_bias, nv},
+      {"qfrc_smooth", &DevData::qfrc_smooth, nv}, {"qacc_smooth", &DevData::qacc_smooth, nv},
+      {"qfrc_constraint", &DevData::qfrc_constraint, nv}, {"qM", &DevData::qM, nv * nv, nv},
+      {"qM_packed", &DevData::qM_packed, m.ntri}, {"qacc_smooth_prev", &DevData::qacc_smooth_prev, nv},
+      {"ctrl_prev", &DevData::ctrl_prev, nu}, {"contact_dist", &DevData::contact_dist, mc},
+      {"contact_pos", &DevData::contact_pos, 3 * mc, 3}, {"contact_frame", &DevData::contact_frame, 9 * mc, 9},
+      {"contact_force", &DevData::contact_force, 3 * mc, 3}, {"solver_cost", &DevData::solver_cost, 1, 0, true}};
+  const DataArray<IArr> ints[] = {
+      {"ncon", &DevData::ncon, 1, 0, true}, {"nefc", &DevData::nefc, 1, 0, true},
+      {"solver_niter", &DevData::solver_niter, 1, 0, true}, {"contact_geom", &DevData::contact_geom, 2 * mc, 2},
+      {"overflow", &DevData::overflow, 1, 0, true}, {"solver_nd", &DevData::solver_nd, 1, 0, true},
+      {"solver_nls", &DevData::solver_nls, 1, 0, true}};  // (solver_nls: line-search derivative evaluations of the last step)
+  for (const auto& r : floats) if (add_data(s, r)) return 1;
+  for (const auto& r : ints) if (add_data(s, r)) return 1;
+  return 0;
+}
 
-  // ---- shared-memory layout (floats per environment) -------------------------------------------
+// Offsets of every region of one environment's shared-memory block (floats per environment), and the kernels'
+// dynamic shared-memory limit.
+static int shared_memory_layout(b2_sim* s, const HostModel& h) {
+  DevModel& m = s->hm;
+  const DevData& d = s->hd;
+  const int nv = m.nv, nu = m.nu, nb = m.nbody, mc = m.maxcon;
   Layout& L = m.lay;
   int off = 0;
   auto alloc = [&](int n) { int o = off; off += pad4(std::max(n, 1)); return o; };
@@ -840,80 +816,92 @@ int b2_create(const B2ModelDesc* desc, int nworld, int ncon_per_world, int njmax
   int endB = off;
   // the lane-distributed height-field narrowphase keeps its owner records and its queue in the (then unused)
   // solver regions from gV on
-  if (!s->mf["hfield_data"].empty()) endB = std::max(endB, L.gV + HF_SCRATCH);
+  if (!h.at(&DevModel::hfield_data).empty()) endB = std::max(endB, L.gV + HF_SCRATCH);
   L.total = pad4(std::max(endA, endB));
   if (L.ndcap == 0) L.Mred = L.H;  // never used
   s->smem_bytes = sizeof(float) * ((size_t)L.total * B2_WARPS_PER_CTA + pad4(m.ldl_nsparse + 18));
-  if (s->smem_bytes > 227 * 1024) {
-    b2_destroy(s);
-    return fail("b2_create: model too large for the per-environment shared-memory block");
+  if (s->smem_bytes > 227 * 1024) return fail("b2_create: model too large for the per-environment shared-memory block");
+  // The attribute is per function and per device, not per sim: only ever raise it, so that an earlier,
+  // larger sim in the same process keeps launching after a smaller one is created.
+  static size_t dev_max[64] = {0};
+  if (s->smem_bytes > dev_max[s->device & 63]) {
+    cudaError_t e1 = cudaFuncSetAttribute(b2_step_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
+    cudaError_t e2 = cudaFuncSetAttribute(b2_step_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
+    if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(b2_step_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
+    if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(b2_step_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
+    if (e1 != cudaSuccess || e2 != cudaSuccess)
+      return fail(std::string("cudaFuncSetAttribute(max dynamic smem): ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    dev_max[s->device & 63] = s->smem_bytes;
   }
-  {
-    // The attribute is per function and per device, not per sim: only ever raise it, so that an earlier,
-    // larger sim in the same process keeps launching after a smaller one is created.
-    static size_t dev_max[64] = {0};
-    if (s->smem_bytes > dev_max[cuda_device & 63]) {
-      cudaError_t e1 = cudaFuncSetAttribute(b2_step_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
-      cudaError_t e2 = cudaFuncSetAttribute(b2_step_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
-      if (e1 == cudaSuccess) e1 = cudaFuncSetAttribute(b2_step_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
-      if (e2 == cudaSuccess) e2 = cudaFuncSetAttribute(b2_step_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->smem_bytes);
-      if (e1 != cudaSuccess || e2 != cudaSuccess) {
-        b2_destroy(s);
-        return fail(std::string("cudaFuncSetAttribute(max dynamic smem): ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
-      }
-      dev_max[cuda_device & 63] = s->smem_bytes;
-    }
-  }
-  {
-    void* p = nullptr;
-    if (cudaMalloc(&p, sizeof(int) * (size_t)nworld) != cudaSuccess) { b2_destroy(s); return fail("cudaMalloc(order)"); }
-    s->allocs.push_back(p);
-    s->order = (int*)p;
-    if (cudaMalloc(&p, sizeof(int) * 4) != cudaSuccess) { b2_destroy(s); return fail("cudaMalloc(tickets)"); }
-    s->allocs.push_back(p);
-    s->tickets = (int*)p;
-    cudaMemset(p, 0, sizeof(int) * 4);
-    int per_sm = 0, sms = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, b2_step_kernel<1>, 32 * B2_WARPS_PER_CTA, s->smem_bytes);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cuda_device);
-    s->resident_ctas = per_sm * sms;
-    for (int h = 0; h < 4; h++) {
-      if (cudaStreamCreateWithFlags(&s->side[h], cudaStreamNonBlocking) != cudaSuccess ||
-          cudaEventCreateWithFlags(&s->ev_join[h], cudaEventDisableTiming) != cudaSuccess) {
-        b2_destroy(s);
-        return fail("b2_create: stream/event creation failed");
-      }
-    }
-    if (cudaEventCreateWithFlags(&s->ev_fork, cudaEventDisableTiming) != cudaSuccess) { b2_destroy(s); return fail("event"); }
-  }
-  // qpos <- qpos0 in every world, then one forward pass so all derived fields are valid
-  {
-    long long total = (long long)nworld * nq;
-    b2_init_rows_kernel<<<(unsigned)((total + 255) / 256), 256>>>(d.qpos.p, d.qpos.stride, m.qpos0.p, nq, nworld);
+  return 0;
+}
+
+// Heavy-first order and work-queue tickets, the step kernel's co-resident CTAs, and the streams of b2_step_n.
+static int launch_resources(b2_sim* s) {
+  void* p = nullptr;
+  if (cudaMalloc(&p, sizeof(int) * (size_t)s->nworld) != cudaSuccess) return fail("cudaMalloc(order)");
+  s->allocs.push_back(p);
+  s->order = (int*)p;
+  if (cudaMalloc(&p, sizeof(int) * 4) != cudaSuccess) return fail("cudaMalloc(tickets)");
+  s->allocs.push_back(p);
+  s->tickets = (int*)p;
+  cudaMemset(p, 0, sizeof(int) * 4);
+  int per_sm = 0, sms = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, b2_step_kernel<1>, 32 * B2_WARPS_PER_CTA, s->smem_bytes);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device);
+  s->resident_ctas = per_sm * sms;
+  for (int h = 0; h < 4; h++)
+    if (cudaStreamCreateWithFlags(&s->side[h], cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&s->ev_join[h], cudaEventDisableTiming) != cudaSuccess)
+      return fail("b2_create: stream/event creation failed");
+  if (cudaEventCreateWithFlags(&s->ev_fork, cudaEventDisableTiming) != cudaSuccess) return fail("event");
+  return 0;
+}
+
+// qpos <- qpos0 in every world, the constant poses of the static geoms, then one forward pass so all derived
+// fields are valid.
+static int first_forward(b2_sim* s) {
+  const DevModel& m = s->hm;
+  const DevData& d = s->hd;
+  const int nworld = s->nworld;
+  long long total = (long long)nworld * m.nq;
+  b2_init_rows_kernel<<<(unsigned)((total + 255) / 256), 256>>>(d.qpos.p, d.qpos.stride, m.qpos0.p, m.nq, nworld);
+  s->launches++;
+  struct { int n; const float* pose; const int* geom; } posed[] = {{m.nstatic, m.static_pose, m.static_geom},
+                                                                   {m.nfixed, m.fixed_pose, m.fixed_geom}};
+  for (const auto& p : posed) {
+    if (p.n == 0) continue;
+    long long tot = (long long)nworld * p.n;
+    b2_static_rows_kernel<<<(unsigned)((tot + 255) / 256), 256>>>(d.geom_xpos.p, d.geom_xpos.stride, d.geom_xmat.p,
+                                                                   d.geom_xmat.stride, p.pose, p.geom, p.n, nworld);
     s->launches++;
-    if (m.nstatic > 0) {
-      long long tot = (long long)nworld * m.nstatic;
-      b2_static_rows_kernel<<<(unsigned)((tot + 255) / 256), 256>>>(d.geom_xpos.p, d.geom_xpos.stride, d.geom_xmat.p,
-                                                                     d.geom_xmat.stride, m.static_pose, m.static_geom,
-                                                                     m.nstatic, nworld);
-      s->launches++;
-    }
-    if (m.nfixed > 0) {
-      long long tot = (long long)nworld * m.nfixed;
-      b2_static_rows_kernel<<<(unsigned)((tot + 255) / 256), 256>>>(d.geom_xpos.p, d.geom_xpos.stride, d.geom_xmat.p,
-                                                                     d.geom_xmat.stride, m.fixed_pose, m.fixed_geom,
-                                                                     m.nfixed, nworld);
-      s->launches++;
-    }
-    if (launch(s, false, 0)) { b2_destroy(s); return 1; }
-    cudaError_t e = cudaDeviceSynchronize();
-    if (e != cudaSuccess) {
-      std::string msg = std::string("b2_create: initial forward failed: ") + cudaGetErrorString(e);
-      b2_destroy(s);
-      return fail(msg);
-    }
   }
-  *out = s;
+  if (launch(s, false, 0)) return 1;
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) return fail(std::string("b2_create: initial forward failed: ") + cudaGetErrorString(e));
+  return 0;
+}
+
+int b2_create(const B2ModelDesc* desc, int nworld, int ncon_per_world, int njmax, int cuda_device,
+              b2_sim** out) {
+  if (!desc || !out || nworld <= 0) return fail("b2_create: bad arguments");
+  HostModel h;
+  std::string why = read_desc(desc, h);
+  if (!why.empty()) return fail("b2_create: " + why);
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+    return fail("b2_create: no CUDA device available (this library has no CPU path)");
+  if (cuda_device < 0 || cuda_device >= ndev) return fail("b2_create: bad cuda_device");
+  DeviceGuard guard(cuda_device);
+  // the sim and everything allocated for it are released on every refusal below; handed out only on success
+  std::unique_ptr<b2_sim, int (*)(b2_sim*)> s(new b2_sim(), b2_destroy);
+  s->device = cuda_device;
+  s->nworld = nworld;
+  if (read_model(desc, ncon_per_world, njmax, h, s->hm) || kinematic_tables(s.get(), h) || collision_plan(s.get(), h) ||
+      upload_model(s.get(), h) || alloc_data(s.get()) || shared_memory_layout(s.get(), h) || launch_resources(s.get()) ||
+      first_forward(s.get()))
+    return 1;
+  *out = s.release();
   return 0;
 }
 
@@ -972,70 +960,78 @@ int b2_expand_model_field(b2_sim* s, const char* name, void* stream, B2Tensor* o
     s->launches++;
     CUDA_OK(cudaGetLastError());
     f->farr->p = (const float*)p; f->farr->stride = n;
-    {
-      std::string nm = name;
-      if (nm == "body_pos" || nm == "body_quat" || nm == "jnt_pos" || nm == "jnt_axis" || nm == "qpos0")
-        s->hm.fastkin = 0;  // the compact kinematic records mirror the shared arrays only
-    }
+    const DevModel& m = s->hm;
+    if (f->farr == &m.body_pos || f->farr == &m.body_quat || f->farr == &m.jnt_pos || f->farr == &m.jnt_axis ||
+        f->farr == &m.qpos0)
+      s->hm.fastkin = 0;  // the compact kinematic records mirror the shared arrays only
     f->ptr = p; f->stride[0] = n;
   }
   if (out) fill_tensor(s, *f, out);
   return 0;
 }
 
+// Options of b2_set_option / b2_get_option.  A value lives in an int or a float of the sim or its model, or in a
+// bit of DevModel::debug; read-only ones report what b2_create derived.  Setting an int or a bit takes (int)value,
+// a bit is set by any non-zero value.
+struct OptionRef { int* i; float* f = nullptr; int bit = 0; double scale = 1.0; };  // *f, bit `bit` of *i, or scale * *i
+struct Option {
+  const char* name;
+  OptionRef (*ref)(b2_sim*);       // nullptr: accepted and ignored
+  bool read_only = false;
+  const char* (*refuse)(double) = nullptr;  // optional: why a value is not taken (nullptr when it is)
+};
+static const Option kOptions[] = {
+    {"iterations", [](b2_sim* s) { return OptionRef{&s->hm.iterations}; }},
+    {"ls_iterations", [](b2_sim* s) { return OptionRef{&s->hm.ls_iterations}; }},
+    {"tolerance", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.tolerance}; }},
+    {"ls_tolerance", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.ls_tolerance}; }},
+    {"timestep", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.timestep}; }},
+    {"integrator", [](b2_sim* s) { return OptionRef{&s->hm.integrator}; }},
+    {"solver", [](b2_sim* s) { return OptionRef{&s->hm.solver}; }, false, [](double v) -> const char* {
+       return (int)v == SOL_NEWTON_ || (int)v == SOL_CG_ ? nullptr : "b2_set_option: solver must be 1 (CG) or 2 (Newton)"; }},
+    {"debug_outputs", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 1}; }},
+    {"dense_factor", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 2}; }},  // force the dense LDL schedule (tests)
+    {"full_solver", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 4}; }},  // Newton on all dofs even when a leading block suffices (tests, A/B)
+    {"ls_relstep", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 8}; }},  // line search stops on a relative step of a few ulp
+    {"warmstart_shift", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 16}; }},  // previous solution moved by the change of qacc_smooth
+    {"ls_eval0", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 32}; }},  // evaluate the line-search slope at 0 instead of using grad . search (A/B)
+    {"ls_rtol", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.ls_rtol}; }},
+    {"newton_small", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.newton_small}; }},
+    {"ls_parallel", nullptr},  // accepted for API parity; the line search here is exact
+    {"sorted_dispatch", [](b2_sim* s) { return OptionRef{&s->sorted_dispatch}; }},
+    {"fused_decimation", [](b2_sim* s) { return OptionRef{&s->fused_decimation}; }},
+    {"split_streams", [](b2_sim* s) { return OptionRef{&s->split_streams}; }},
+    {"work_queue", [](b2_sim* s) { return OptionRef{&s->work_queue}; }}, {"phase_sync", [](b2_sim* s) { return OptionRef{&s->phase_sync}; }},
+    {"reorder_every_substep", [](b2_sim* s) { return OptionRef{&s->reorder_every_substep}; }},
+    {"smem_bytes_per_env", [](b2_sim* s) { return OptionRef{&s->hm.lay.total, nullptr, 0, 4.0}; }, true},
+    {"maxcon", [](b2_sim* s) { return OptionRef{&s->hm.maxcon}; }, true},
+    {"resident_ctas", [](b2_sim* s) { return OptionRef{&s->resident_ctas}; }, true},
+    {"reduced_block_cap", [](b2_sim* s) { return OptionRef{&s->hm.lay.ndcap}; }, true}};
+
+static const Option* find_option(const char* key) {
+  for (const Option& o : kOptions)
+    if (!strcmp(o.name, key)) return &o;
+  return nullptr;
+}
+
 int b2_set_option(b2_sim* s, const char* key, double v) {
   if (!s || !key) return fail("b2_set_option: bad arguments");
-  std::string k = key;
-  DevModel& m = s->hm;
-  if (k == "iterations") m.iterations = (int)v;
-  else if (k == "ls_iterations") m.ls_iterations = (int)v;
-  else if (k == "tolerance") m.tolerance = (float)v;
-  else if (k == "ls_tolerance") m.ls_tolerance = (float)v;
-  else if (k == "timestep") m.timestep = (float)v;
-  else if (k == "integrator") m.integrator = (int)v;
-  else if (k == "solver") {
-    if ((int)v != SOL_NEWTON_ && (int)v != SOL_CG_) return fail("b2_set_option: solver must be 1 (CG) or 2 (Newton)");
-    m.solver = (int)v;
-  }
-  else if (k == "debug_outputs") m.debug = (m.debug & ~1) | ((int)v & 1);
-  else if (k == "dense_factor") m.debug = (m.debug & ~2) | ((int)v ? 2 : 0);  // force the dense LDL schedule (tests)
-  else if (k == "ls_parallel") { /* accepted for API parity; the line search here is exact */ }
-  else if (k == "sorted_dispatch") s->sorted_dispatch = (int)v;
-  else if (k == "fused_decimation") s->fused_decimation = (int)v;
-  else if (k == "split_streams") s->split_streams = (int)v;
-  else if (k == "work_queue") s->work_queue = (int)v;
-  else if (k == "phase_sync") s->phase_sync = (int)v;
-  else if (k == "reorder_every_substep") s->reorder_every_substep = (int)v;
-  else if (k == "full_solver") m.debug = (m.debug & ~4) | ((int)v ? 4 : 0);  // Newton on all dofs even when a leading block suffices (tests, A/B)
-  else if (k == "warmstart_shift") m.debug = (m.debug & ~16) | ((int)v ? 16 : 0);  // previous solution moved by the change of qacc_smooth
-  else if (k == "ls_rtol") m.ls_rtol = (float)v;
-  else if (k == "ls_eval0") m.debug = (m.debug & ~32) | ((int)v ? 32 : 0);  // evaluate the line-search slope at 0 instead of using grad . search (A/B)
-  else if (k == "newton_small") m.newton_small = (float)v;
-  else if (k == "ls_relstep") m.debug = (m.debug & ~8) | ((int)v ? 8 : 0);  // line search stops on a relative step of a few ulp
-  else return fail("b2_set_option: unknown option '" + k + "'");
+  const Option* o = find_option(key);
+  if (!o || o->read_only) return fail(std::string("b2_set_option: unknown option '") + key + "'");
+  if (o->refuse && o->refuse(v)) return fail(o->refuse(v));
+  if (!o->ref) return 0;
+  OptionRef r = o->ref(s);
+  if (r.f) *r.f = (float)v;
+  else if (r.bit) *r.i = (*r.i & ~r.bit) | ((int)v ? r.bit : 0);
+  else *r.i = (int)v;
   return 0;
 }
 int b2_get_option(b2_sim* s, const char* key, double* v) {
   if (!s || !key || !v) return fail("b2_get_option: bad arguments");
-  std::string k = key;
-  const DevModel& m = s->hm;
-  if (k == "iterations") *v = m.iterations;
-  else if (k == "ls_iterations") *v = m.ls_iterations;
-  else if (k == "tolerance") *v = m.tolerance;
-  else if (k == "ls_tolerance") *v = m.ls_tolerance;
-  else if (k == "timestep") *v = m.timestep;
-  else if (k == "integrator") *v = m.integrator;
-  else if (k == "solver") *v = m.solver;
-  else if (k == "debug_outputs") *v = m.debug & 1;
-  else if (k == "dense_factor") *v = (m.debug >> 1) & 1;
-  else if (k == "smem_bytes_per_env") *v = 4.0 * m.lay.total;
-  else if (k == "maxcon") *v = m.maxcon;
-  else if (k == "full_solver") *v = (m.debug >> 2) & 1;
-  else if (k == "work_queue") *v = s->work_queue;
-  else if (k == "phase_sync") *v = s->phase_sync;
-  else if (k == "resident_ctas") *v = s->resident_ctas;
-  else if (k == "reduced_block_cap") *v = m.lay.ndcap;
-  else return fail("b2_get_option: unknown option '" + k + "'");
+  const Option* o = find_option(key);
+  if (!o || !o->ref) return fail(std::string("b2_get_option: unknown option '") + key + "'");
+  OptionRef r = o->ref(s);
+  *v = r.f ? (double)*r.f : r.bit ? (double)((*r.i & r.bit) != 0) : r.scale * *r.i;
   return 0;
 }
 

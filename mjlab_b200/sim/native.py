@@ -3,13 +3,13 @@
 from __future__ import annotations
 
 import ctypes
+import math
+import os
 from pathlib import Path
 
 import numpy as np
 
 from mjlab_b200.compiler.compile import MODEL_ARRAYS, MODEL_SCALARS_F, MODEL_SCALARS_I, fill_asset_defaults
-
-import os
 
 LIB_PATH = Path(os.environ.get("B2SIM_LIB") or Path(__file__).resolve().parents[1] / "csrc" / "libb2sim.so")
 
@@ -98,6 +98,42 @@ def make_model_desc(model):
   return desc, keep
 
 
+def bind(L: ctypes.CDLL) -> ctypes.CDLL:
+  """Declare the signature of every entry point of include/b2sim.h on ``L`` (the CUDA library or its host emulation).
+
+  Without ``argtypes`` ctypes passes a Python int as a C ``int``, which truncates a 64-bit pointer."""
+  vp, ci, cd, cs = ctypes.c_void_p, ctypes.c_int, ctypes.c_double, ctypes.c_char_p
+  P = ctypes.POINTER
+  signatures = {
+    "b2_create": ([P(B2ModelDesc), ci, ci, ci, ci, P(vp)], ci),
+    "b2_destroy": ([vp], ci),
+    "b2_get_field": ([vp, ci, cs, P(B2Tensor)], ci),
+    "b2_num_fields": ([vp, ci], ci),
+    "b2_field_name": ([vp, ci, ci], cs),
+    "b2_expand_model_field": ([vp, cs, vp, P(B2Tensor)], ci),
+    "b2_set_option": ([vp, cs, cd], ci),
+    "b2_get_option": ([vp, cs, P(cd)], ci),
+    "b2_step": ([vp, vp], ci),
+    "b2_forward": ([vp, vp], ci),
+    "b2_step_n": ([vp, ci, vp], ci),
+    "b2_forward_masked": ([vp, vp, vp], ci),
+    "b2_step_host": ([vp, vp, ci, vp, vp, vp], ci),
+    "b2_velenv_pre": ([vp, vp, vp, vp, vp], ci),
+    "b2_velenv_post": ([vp, P(B2VelEnvArgs), vp], ci),
+    "b2_trackenv_post1": ([vp, P(B2TrackEnvArgs), vp], ci),
+    "b2_trackenv_post2": ([vp, P(B2TrackEnvArgs), vp], ci),
+    "b2_stats": ([vp, vp, P(B2Stats)], ci),
+    "b2_launch_count": ([vp], ctypes.c_int64),
+    "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),
+    "b2_last_error": ([], cs),
+    "b2_version": ([], cs),
+  }
+  for name, (args, res) in signatures.items():
+    fn = getattr(L, name)
+    fn.argtypes, fn.restype = args, res
+  return L
+
+
 _lib = None
 
 
@@ -111,36 +147,66 @@ def load_library() -> ctypes.CDLL:
       f"{LIB_PATH} not found: build the CUDA extension first "
       "(python -c 'import __graft_entry__ as g; g.build()'). There is no CPU fallback."
     )
-  L = ctypes.CDLL(str(LIB_PATH))
-  L.b2_last_error.restype = ctypes.c_char_p
-  L.b2_version.restype = ctypes.c_char_p
-  L.b2_field_name.restype = ctypes.c_char_p
-  L.b2_launch_count.restype = ctypes.c_int64
-  vp, ci, cd = ctypes.c_void_p, ctypes.c_int, ctypes.c_double
-  L.b2_create.argtypes = [ctypes.POINTER(B2ModelDesc), ci, ci, ci, ci, ctypes.POINTER(vp)]
-  L.b2_destroy.argtypes = [vp]
-  L.b2_get_field.argtypes = [vp, ci, ctypes.c_char_p, ctypes.POINTER(B2Tensor)]
-  L.b2_num_fields.argtypes = [vp, ci]
-  L.b2_field_name.argtypes = [vp, ci, ci]
-  L.b2_expand_model_field.argtypes = [vp, ctypes.c_char_p, vp, ctypes.POINTER(B2Tensor)]
-  L.b2_set_option.argtypes = [vp, ctypes.c_char_p, cd]
-  L.b2_get_option.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(cd)]
-  L.b2_step.argtypes = [vp, vp]
-  L.b2_forward.argtypes = [vp, vp]
-  L.b2_step_n.argtypes = [vp, ci, vp]
-  L.b2_forward_masked.argtypes = [vp, vp, vp]
-  L.b2_velenv_pre.argtypes = [vp, vp, vp, vp, vp]
-  L.b2_velenv_post.argtypes = [vp, ctypes.POINTER(B2VelEnvArgs), vp]
-  L.b2_trackenv_post1.argtypes = [vp, ctypes.POINTER(B2TrackEnvArgs), vp]
-  L.b2_trackenv_post2.argtypes = [vp, ctypes.POINTER(B2TrackEnvArgs), vp]
-  L.b2_step_host.argtypes = [vp, vp, ci, vp, vp, vp]
-  L.b2_stats.argtypes = [vp, vp, ctypes.POINTER(B2Stats)]
-  L.b2_launch_count.argtypes = [vp]
-  L.b2_algorithmic_bytes.argtypes = [vp, vp, ctypes.POINTER(cd), ctypes.POINTER(cd)]
-  _lib = L
-  return L
+  _lib = bind(ctypes.CDLL(str(LIB_PATH)))
+  return _lib
 
 
 def check(rc: int) -> None:
   if rc != 0:
     raise RuntimeError(f"b2sim: {load_library().b2_last_error().decode()}")
+
+
+def ncon_per_world(nconmax: int | None, nworld: int) -> int:
+  """Per-world contact capacity for upstream's global ``nconmax`` pool (SURVEY.md App. C); 0: the engine's default."""
+  if nconmax is None:
+    return 0
+  return max(16, min(96, math.ceil(nconmax / max(nworld, 1))))
+
+
+class Engine:
+  """One ``b2_sim`` of a bound library (the CUDA library or its host emulation): created with the contact-capacity
+  rule and destroyed once, with its field names, field descriptors and options.  Errors are read from the library
+  that made the sim.  Subclasses wrap fields as tensors (device or host memory) and pick the stream."""
+
+  def __init__(self, lib: ctypes.CDLL, model, nworld: int, nconmax: int | None = None, njmax: int | None = None,
+               cuda_device: int = 0):
+    self.lib = lib
+    self.nworld = int(nworld)
+    self.h = None
+    desc, self._keep = make_model_desc(model)
+    h = ctypes.c_void_p()
+    self.check(lib.b2_create(ctypes.byref(desc), self.nworld, ncon_per_world(nconmax, self.nworld), int(njmax or 0),
+                             cuda_device, ctypes.byref(h)))
+    self.h = h
+
+  def check(self, rc: int) -> None:
+    if rc != 0:
+      raise RuntimeError(f"b2sim: {self.lib.b2_last_error().decode()}")
+
+  def names(self, which: int) -> list[str]:
+    return [self.lib.b2_field_name(self.h, which, i).decode() for i in range(self.lib.b2_num_fields(self.h, which))]
+
+  def get_field(self, which: int, name: str) -> B2Tensor:
+    t = B2Tensor()
+    self.check(self.lib.b2_get_field(self.h, which, name.encode(), ctypes.byref(t)))
+    return t
+
+  def set_option(self, key: str, value: float) -> None:
+    self.check(self.lib.b2_set_option(self.h, key.encode(), float(value)))
+
+  def get_option(self, key: str) -> float:
+    v = ctypes.c_double()
+    self.check(self.lib.b2_get_option(self.h, key.encode(), ctypes.byref(v)))
+    return v.value
+
+  def close(self) -> None:
+    if self.h:
+      self.lib.b2_destroy(self.h)
+      self.h = None
+
+  def __del__(self):
+    # Tensors handed out keep their owner alive, so this only runs once no view of engine memory exists any more.
+    try:
+      self.close()
+    except Exception:
+      pass

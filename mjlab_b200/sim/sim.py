@@ -11,7 +11,6 @@ extension, raises.
 from __future__ import annotations
 
 import ctypes
-import math
 from dataclasses import dataclass, field
 from types import SimpleNamespace
 from typing import Any, Literal
@@ -76,23 +75,15 @@ class Simulation:
     if not torch.cuda.is_available():
       raise RuntimeError("Simulation: no CUDA device is available")
     self._dev_index = dev.index if dev.index is not None else torch.cuda.current_device()
-    self._lib = native.load_library()
     self._mj_model = model
     self._mj_data = SimpleNamespace(
       qpos=np.array(model.qpos0, dtype=np.float64), qvel=np.zeros(int(model.nv)), time=0.0
     )
-    # `nconmax` is a global pool upstream (SURVEY.md App. C); here it becomes a per-world capacity
-    ncon = 0
-    if cfg.nconmax is not None:
-      ncon = max(16, min(96, math.ceil(cfg.nconmax / max(num_envs, 1))))
-    njmax = cfg.njmax or 0
-    desc, self._keep = native.make_model_desc(model)
-    h = ctypes.c_void_p()
+    lib = native.load_library()
     torch.cuda.synchronize(self._dev_index)
-    native.check(
-      self._lib.b2_create(ctypes.byref(desc), num_envs, ncon, njmax, self._dev_index, ctypes.byref(h))
-    )
-    self._h = h
+    self._engine = native.Engine(lib, model, num_envs, cfg.nconmax, cfg.njmax, self._dev_index)
+    # the env drivers launch their kernels on this library and sim
+    self._lib, self._h = lib, self._engine.h
     self.set_option("ls_parallel", float(cfg.ls_parallel))
 
     opt = SimpleNamespace(
@@ -120,12 +111,10 @@ class Simulation:
     return ctypes.c_void_p(torch.cuda.current_stream(self._dev_index).cuda_stream)
 
   def set_option(self, key: str, value: float) -> None:
-    native.check(self._lib.b2_set_option(self._h, key.encode(), float(value)))
+    self._engine.set_option(key, value)
 
   def get_option(self, key: str) -> float:
-    v = ctypes.c_double()
-    native.check(self._lib.b2_get_option(self._h, key.encode(), ctypes.byref(v)))
-    return v.value
+    return self._engine.get_option(key)
 
   def create_graph(self) -> None:
     """Capture ``step`` and ``forward`` as CUDA graphs (reference ``sim.py:131-140``)."""
@@ -242,16 +231,5 @@ class Simulation:
         st._tensors.clear()
         st._closed = True
         object.__getattribute__(br, "_wrapped_cache").clear()
-      self._lib.b2_destroy(h)
+      self._engine.close()
       self._h = None
-
-  def __del__(self):
-    # Tensors handed out keep `self` alive through _RawCudaBuffer, so this only runs once no view
-    # of engine memory exists any more.
-    try:
-      h = getattr(self, "_h", None)
-      if h:
-        self._lib.b2_destroy(h)
-        self._h = None
-    except Exception:
-      pass

@@ -9,7 +9,6 @@ enqueued on torch's *current* stream, so writes through ``__setitem__`` need no 
 
 from __future__ import annotations
 
-import ctypes
 from typing import Any, Dict, Optional, Tuple
 
 import torch
@@ -154,10 +153,7 @@ class EngineStruct:
     self._which = which
     self._tensors: dict[str, torch.Tensor] = {}
     self._extra = extra or {}
-    lib = sim._lib
-    self._names = [
-      lib.b2_field_name(sim._h, which, i).decode() for i in range(lib.b2_num_fields(sim._h, which))
-    ]
+    self._names = sim._engine.names(which)
 
   def __getattr__(self, name: str) -> Any:
     if name.startswith("_"):
@@ -170,9 +166,7 @@ class EngineStruct:
       return self._tensors[name]
     if name not in self._names:
       raise AttributeError(f"engine struct has no field '{name}'")
-    t = native.B2Tensor()
-    native.check(self._sim._lib.b2_get_field(self._sim._h, self._which, name.encode(), ctypes.byref(t)))
-    tensor = tensor_from_b2(t, self._sim)
+    tensor = tensor_from_b2(self._sim._engine.get_field(self._which, name), self._sim)
     self._tensors[name] = tensor
     return tensor
 

@@ -6,7 +6,6 @@ Lets the CPU suite run the reference's own ``Simulation`` / ``Entity`` / event c
 start without a CUDA device.
 """
 import ctypes
-import math
 import sys
 from pathlib import Path
 
@@ -23,23 +22,7 @@ _LIB = None
 def load_emul_library(defines=()):
   from build import build
 
-  L = ctypes.CDLL(str(build(defines=defines)))
-  L.b2_last_error.restype = ctypes.c_char_p
-  vp, ci = ctypes.c_void_p, ctypes.c_int
-  L.b2_create.argtypes = [ctypes.POINTER(native.B2ModelDesc), ci, ci, ci, ci, ctypes.POINTER(vp)]
-  L.b2_destroy.argtypes = [vp]
-  L.b2_get_field.argtypes = [vp, ci, ctypes.c_char_p, ctypes.POINTER(native.B2Tensor)]
-  L.b2_set_option.argtypes = [vp, ctypes.c_char_p, ctypes.c_double]
-  L.b2_get_option.argtypes = [vp, ctypes.c_char_p, ctypes.POINTER(ctypes.c_double)]
-  L.b2_step.argtypes = [vp, vp]
-  L.b2_forward.argtypes = [vp, vp]
-  L.b2_step_n.argtypes = [vp, ci, vp]
-  L.b2_forward_masked.argtypes = [vp, vp, vp]
-  L.b2_expand_model_field.argtypes = [vp, ctypes.c_char_p, vp, ctypes.POINTER(native.B2Tensor)]
-  L.b2_num_fields.argtypes = [vp, ci]
-  L.b2_field_name.argtypes = [vp, ci, ci]
-  L.b2_field_name.restype = ctypes.c_char_p
-  return L
+  return native.bind(ctypes.CDLL(str(build(defines=defines))))
 
 
 def host_tensor(t: native.B2Tensor) -> torch.Tensor:
@@ -55,44 +38,19 @@ def host_tensor(t: native.B2Tensor) -> torch.Tensor:
   return flat.as_strided(shape, stride)
 
 
-class EmulEngine:
-  """Drop-in for ``_Engine`` (lib / h / nworld / device / names / tensor / stream)."""
+class EmulEngine(native.Engine):
+  """Drop-in for ``_Engine`` (lib / h / nworld / device / names / tensor / stream) on the emulated library."""
 
   def __init__(self, mjm, nworld: int, nconmax, njmax):
     global _LIB
     if _LIB is None:
       _LIB = load_emul_library()
-    self.lib = _LIB
-    self.nworld = int(nworld)
+    super().__init__(_LIB, mjm, nworld, nconmax, njmax)
     self.device = "cpu"
-    ncon = 0
-    if nconmax is not None:
-      ncon = max(16, min(96, math.ceil(nconmax / max(nworld, 1))))
-    desc, self._keep = native.make_model_desc(mjm)
-    h = ctypes.c_void_p()
-    rc = self.lib.b2_create(ctypes.byref(desc), self.nworld, ncon, int(njmax or 0), 0, ctypes.byref(h))
-    if rc:
-      raise RuntimeError(self.lib.b2_last_error(None).decode())
-    self.h = h
-    self.lib.b2_set_option(h, b"sorted_dispatch", 0.0)  # (the 1024-thread sort kernel is slow to emulate)
-
-  def names(self, which: int):
-    return [self.lib.b2_field_name(self.h, which, i).decode() for i in range(self.lib.b2_num_fields(self.h, which))]
+    self.set_option("sorted_dispatch", 0.0)  # (the 1024-thread sort kernel is slow to emulate)
 
   def tensor(self, which: int, name: str) -> torch.Tensor:
-    t = native.B2Tensor()
-    rc = self.lib.b2_get_field(self.h, which, name.encode(), ctypes.byref(t))
-    if rc:
-      raise RuntimeError(self.lib.b2_last_error(self.h).decode())
-    return host_tensor(t)
+    return host_tensor(self.get_field(which, name))
 
   def stream(self) -> ctypes.c_void_p:
     return ctypes.c_void_p(0)
-
-  def __del__(self):
-    try:
-      if self.h:
-        self.lib.b2_destroy(self.h)
-        self.h = None
-    except Exception:
-      pass

@@ -24,8 +24,12 @@ def test_c_abi_exports_every_declared_symbol():
   lib = ctypes.CDLL(str(ROOT / "mjlab_b200" / "csrc" / "libb2sim.so"))
   for sym in declared:
     assert hasattr(lib, sym), f"{sym} declared in include/b2sim.h but not exported"
-  lib.b2_version.restype = ctypes.c_char_p
+  from mjlab_b200.sim import native
+
+  native.bind(lib)
   assert b"sm_90a" in lib.b2_version()
+  bound = {name for name in declared if getattr(lib, name).argtypes is not None}
+  assert bound == declared  # native.bind gives every entry point of the header its signature
 
 
 def test_library_is_built_for_sm_90a_with_tma():
@@ -153,27 +157,33 @@ def test_shard_range():
 
 def test_b2_create_rejects_malformed_model_tables(g1_model):
   """The descriptor is validated on the host before any device work: wrong sizes and out-of-range indices are
-  refused with a message (no compute happens here; on a CPU box a valid table ends at 'no CUDA device')."""
+  refused with a message (no compute happens here; on a CPU box a valid table ends at 'no CUDA device').  Models
+  that pass these checks but that the engine does not support are refused later in b2_create; those refusals run on
+  the host-emulated library (tests/emul), where b2_create gets past the device check."""
   import copy
-  import ctypes
+  import sys
 
   import numpy as np
 
+  from mjlab_b200.asset_zoo import load_compiled
   from mjlab_b200.sim import native
 
-  lib = native.load_library()
-  lib.b2_last_error.restype = ctypes.c_char_p
-
-  def create(model):
+  def create(lib, model):
     desc, keep = native.make_model_desc(model)
     h = ctypes.c_void_p()
     rc = lib.b2_create(ctypes.byref(desc), 2, 0, 0, 0, ctypes.byref(h))
-    msg = lib.b2_last_error(None).decode() if rc else ""
+    msg = lib.b2_last_error().decode() if rc else ""
     if rc == 0:
       lib.b2_destroy(h)
     return rc, msg
 
-  rc, msg = create(g1_model)
+  def edit(model, field, mod):
+    m2 = copy.deepcopy(model)
+    m2.arrays[field] = np.ascontiguousarray(mod(np.asarray(model.arrays[field]).reshape(-1)))
+    return m2
+
+  lib = native.load_library()
+  rc, msg = create(lib, g1_model)
   assert rc == 0 or "no CUDA device" in msg  # the unmodified table passes validation
   cases = [
     ("dof_parentid", lambda a: a[:-1], "has 34 elements, expected 35"),
@@ -182,9 +192,28 @@ def test_b2_create_rejects_malformed_model_tables(g1_model):
     ("body_parentid", lambda a: np.where(np.arange(len(a)) == 2, 5, a).astype(np.int32), "parents must precede children"),
   ]
   for field, mod, expect in cases:
-    m2 = copy.deepcopy(g1_model)
-    m2.arrays[field] = np.ascontiguousarray(mod(np.asarray(g1_model.arrays[field])))
-    rc, msg = create(m2)
+    rc, msg = create(lib, edit(g1_model, field, mod))
+    assert rc != 0 and expect in msg, (field, msg)
+
+  sys.path.insert(0, str(ROOT / "tests" / "emul"))
+  from engine import load_emul_library
+
+  emul = load_emul_library()
+  stairs = load_compiled("go1_stairs_small")
+  robot_geom = int(np.asarray(g1_model.arrays["pair_geom2"])[0])  # a foot, on a moving body
+  grid_params = np.asarray(stairs.arrays["grid_params"])
+  late = [
+    (g1_model, "geom_type", lambda a: np.where(np.arange(len(a)) == robot_geom, 0, a).astype(np.int32),
+     "collision pair with an unsupported geom type combination"),  # plane against plane
+    (g1_model, "sensor_intprm", lambda a: np.where(np.arange(len(a)) == 0, 4, a).astype(np.int32),
+     "contact sensor data/reduce combination not implemented"),
+    (stairs, "static_geom", lambda a: np.where(np.arange(len(a)) == 0, int(np.asarray(stairs.arrays["ngeom"])) - 1, a).astype(np.int32),
+     "grid-static geoms must sit on a jointless child of the world body"),
+    (stairs, "grid_params", lambda a: a[:-1], "array 'grid_params' has 4 elements, expected 5"),
+  ]
+  assert create(emul, stairs) == (0, "") and grid_params.size == 5
+  for model, field, mod, expect in late:
+    rc, msg = create(emul, edit(model, field, mod))
     assert rc != 0 and expect in msg, (field, msg)
 
 

@@ -28,22 +28,19 @@ def lib():
   return _load()
 
 
-class EmulSim:
-  """ctypes + numpy views over the emulated library ("device" memory is host memory)."""
+class EmulSim(native.Engine):
+  """numpy views over the emulated library ("device" memory is host memory); `ncon`: contacts per world (16..96)."""
 
   def __init__(self, lib, model, nworld, ncon=0):
-    self.lib, self.n = lib, nworld
-    self.desc, self._keep = native.make_model_desc(model)
-    self.h = ctypes.c_void_p()
-    rc = lib.b2_create(ctypes.byref(self.desc), nworld, ncon, 0, 0, ctypes.byref(self.h))
-    assert rc == 0, lib.b2_last_error(None).decode()
-    lib.b2_set_option(self.h, b"debug_outputs", 1.0)
-    lib.b2_set_option(self.h, b"sorted_dispatch", 0.0)  # (the 1024-thread sort kernel works but is slow to emulate)
+    super().__init__(lib, model, nworld, nconmax=ncon * nworld if ncon else None)
+    self.n = nworld
+    self.set_option("debug_outputs", 1.0)
+    self.set_option("sorted_dispatch", 0.0)  # (the 1024-thread sort kernel works but is slow to emulate)
+
+  option = native.Engine.get_option
 
   def field(self, name, which=0):
-    t = native.B2Tensor()
-    rc = self.lib.b2_get_field(self.h, which, name.encode(), ctypes.byref(t))
-    assert rc == 0, name
+    t = self.get_field(which, name)
     dt = {0: np.float32, 1: np.int32}[t.dtype] if t.dtype in (0, 1) else np.float32
     shape = tuple(t.shape[i] for i in range(t.ndim))
     strides = tuple(t.stride[i] * 4 for i in range(t.ndim))
@@ -55,19 +52,11 @@ class EmulSim:
     for k, v in st.items():
       self.field(k)[...] = v
 
-  def option(self, key):
-    v = ctypes.c_double()
-    self.lib.b2_get_option(self.h, key.encode(), ctypes.byref(v))
-    return v.value
-
   def forward(self):
     assert self.lib.b2_forward(self.h, None) == 0
 
   def step(self, n=1):
     assert self.lib.b2_step_n(self.h, n, None) == 0
-
-  def close(self):
-    self.lib.b2_destroy(self.h)
 
 
 def _check_forward(sim, o, n, acc_tol=1e-3):
@@ -200,8 +189,6 @@ def test_emulated_host_entry_fused_decimation_and_field_expansion(lib):
   (geom_friction) is what the kernel reads."""
   from mjlab_b200.asset_zoo import load_compiled
 
-  lib.b2_step_host.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-  lib.b2_expand_model_field.argtypes = [ctypes.c_void_p, ctypes.c_char_p, ctypes.c_void_p, ctypes.POINTER(native.B2Tensor)]
   m = load_compiled("go1_flat")
   n, nq, nv, nu = 3, int(m.nq), int(m.nv), int(m.nu)
   st = make_states(m, n, seed=21)
@@ -247,13 +234,7 @@ class EmulSimulation:
 
     self._torch = torch
     self._lib = _load()
-    vp = ctypes.c_void_p
-    self._lib.b2_velenv_pre.argtypes = [vp, vp, vp, vp, vp]
-    self._lib.b2_velenv_post.argtypes = [vp, ctypes.POINTER(native.B2VelEnvArgs), vp]
-    self._lib.b2_expand_model_field.argtypes = [vp, ctypes.c_char_p, vp, ctypes.POINTER(native.B2Tensor)]
-    self._lib.b2_trackenv_post1.argtypes = [vp, ctypes.POINTER(native.B2TrackEnvArgs), vp]
-    self._lib.b2_trackenv_post2.argtypes = [vp, ctypes.POINTER(native.B2TrackEnvArgs), vp]
-    self._e = EmulSim(self._lib, model, num_envs, ncon=max(16, min(96, -(-cfg.nconmax // num_envs))) if cfg.nconmax else 0)
+    self._e = EmulSim(self._lib, model, num_envs, ncon=native.ncon_per_world(cfg.nconmax, num_envs))
     self._h = self._e.h
     self.device = device
     outer = self
@@ -265,7 +246,7 @@ class EmulSimulation:
       def __getattr__(self, name):
         try:
           return outer._torch.from_numpy(outer._e.field(name, which=self._which))
-        except AssertionError:
+        except RuntimeError:  # (unknown field)
           raise AttributeError(name) from None
 
     self.data, self.model = _Fields(0), _Fields(1)
@@ -501,3 +482,28 @@ def test_emulated_sorted_dispatch_changes_scheduling_only(lib):
     sim.close()
   assert len(np.unique(out[0][2])) > 2  # the sort key (Newton iterations) takes several values
   assert np.array_equal(out[0][0], out[1][0]) and np.array_equal(out[0][1], out[1][1])
+
+
+def test_emulated_options_read_back(lib):
+  """Every option b2_set_option takes reads back through b2_get_option, except `ls_parallel` (accepted for API parity
+  and ignored); the sizes b2_create derives can be read but not set."""
+  from mjlab_b200.asset_zoo import load_compiled
+
+  sim = EmulSim(lib, load_compiled("go1_flat"), 2)
+  values = dict(iterations=7, ls_iterations=9, tolerance=0.25, ls_tolerance=0.125, timestep=0.00390625, integrator=0,
+                solver=1, debug_outputs=0, dense_factor=1, full_solver=1, ls_relstep=0, warmstart_shift=0, ls_eval0=0,
+                ls_rtol=0.5, newton_small=0.0625, sorted_dispatch=1, fused_decimation=1, split_streams=3, work_queue=1,
+                phase_sync=1, reorder_every_substep=0)
+  for k, v in values.items():
+    assert sim.option(k) != v, k  # (a value other than the current one, so that the set is seen)
+    sim.set_option(k, v)
+    assert sim.option(k) == v, k
+  sim.set_option("ls_parallel", 0.0)
+  with pytest.raises(RuntimeError, match="unknown option 'ls_parallel'"):
+    sim.option("ls_parallel")
+  for k in ("smem_bytes_per_env", "maxcon", "resident_ctas", "reduced_block_cap"):
+    v = sim.option(k)
+    with pytest.raises(RuntimeError, match=f"b2_set_option: unknown option '{k}'"):
+      sim.set_option(k, v + 1)
+    assert sim.option(k) == v
+  sim.close()

@@ -18,6 +18,7 @@ import pytest
 import torch
 
 import refload
+from mjlab_b200.sim import native
 from util import load_oracle, make_states, relerr
 
 pytestmark = [pytest.mark.skipif(not refload.available(), reason="oracle/_ref not installed")]
@@ -38,7 +39,6 @@ def DEV(request, ref):
     yield "cuda:0"
     return
   import mjlab_b200.compat.mujoco_warp_shim as mw
-  from mjlab_b200.sim import native
 
   sys.path.insert(0, str(Path(__file__).parent / "emul"))
   from engine import EmulEngine
@@ -106,7 +106,7 @@ def test_reference_simulation_steps_the_engine(ref, world, DEV):
     assert not sim.use_cuda_graph and sim.step_graph is None
   st = make_states(m, N, seed=77)
   mine = Simulation(N, SimulationCfg(nconmax=140_000 * N // 4096 + 64 * N, njmax=300), m, DEV) if gpu else None
-  maxcon = int(mine.get_option("maxcon")) if gpu else max(16, min(96, -(-(140_000 * N // 4096 + 64 * N) // N)))
+  maxcon = int(mine.get_option("maxcon")) if gpu else native.ncon_per_world(140_000 * N // 4096 + 64 * N, N)
   o = Oracle(m, nworld=N, maxcon=maxcon)
   load_oracle(o, st)
   _load_state(sim, st, DEV)
