@@ -147,8 +147,14 @@ int b2_velenv_post(b2_sim* sim, const B2VelEnvArgs* args, void* cuda_stream);
  * b2_forward_masked; post2 runs after that forward (anchor-relative targets, interval push, observations).
  * Per-step uniforms U[n][B2_TRACKENV_NU(nu)]: with S = 13 + nu, [0, S) reset block (0 clip frame, 1-6 pose noise,
  * 7-12 velocity noise, 13.. joint noise), [S, 2S) the same for envs that ran off the clip, [2S, 2S+7) push (6
- * velocity + timer), then observation noise: anchor pos 3, anchor ori 6, base lin 3, base ang 3, joint pos nu, joint vel nu. */
+ * velocity + timer), then observation noise: anchor pos 3, anchor ori 6, base lin 3, base ang 3, joint pos nu, joint vel nu.
+ * Start frames of resets and clip restarts (B2TrackEnvArgs.adaptive) come from the block's first uniform u:
+ *   B2_START_UNIFORM   floor(u (T-1));
+ *   B2_START_ADAPTIVE  the failure-bin sampler of commands.py:256-297: bin = first b with cdf[b] > u, frac = its
+ *                      position inside that bin's CDF step, frame = floor((bin + frac) / nbins (T-1));
+ *   B2_START_FIRST     frame 0 (disable_adaptive_sampling, the reference's play mode). */
 #define B2_TRACKENV_NU(nu) (48 + 4 * (nu))
+enum { B2_START_UNIFORM = 0, B2_START_ADAPTIVE = 1, B2_START_FIRST = 2 };
 typedef struct B2TrackEnvArgs {
   const float* action;            /* [n][nu] */
   const float* U;                 /* [n][B2_TRACKENV_NU(nu)] */
@@ -180,9 +186,23 @@ typedef struct B2TrackEnvArgs {
   float pose_range[12], vel_range[12]; /* (lo, hi) x 6 */
   float step_dt, jp_lo, jp_hi, push_lo, push_hi;
   int32_t nb, nee, anchor, T, self_collision_adr, root_body, max_episode_length;
+  /* start-frame sampler; a zeroed tail is B2_START_UNIFORM and leaves every field below unread */
+  const float* adaptive_kernel;   /* [adaptive_kernel_size] smoothing weights lambda^i / sum (commands.py:106-110) */
+  float* cdf;                     /* [nbins] in/out: CDF of the start-bin distribution post1 draws from */
+  float* bin_fail_ema;            /* [nbins] in/out: EMA of terminations per bin (bin_failed_count) */
+  float* bin_fail_cur;            /* [nbins] in/out: terminations per bin in this env step (_current_bin_failed) */
+  float* metrics;                 /* [3] out: normalised entropy, top-1 probability, top-1 bin / nbins of the
+                                     distribution this env step's draws used (1, p, b / nbins for one bin) */
+  float adaptive_alpha, adaptive_uniform_ratio;
+  int32_t nbins, adaptive, adaptive_kernel_size;
 } B2TrackEnvArgs;
 int b2_trackenv_post1(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
 int b2_trackenv_post2(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
+/* B2_START_ADAPTIVE only, between post1 and the masked forward (one CTA): metrics of the distribution post1 drew
+ * from, bin_fail_ema = alpha bin_fail_cur + (1 - alpha) bin_fail_ema, bin_fail_cur = 0, then the CDF of the next
+ * env step's distribution p ~ conv1d(replicate_pad(bin_fail_ema + ratio / nbins), kernel), prefix-summed in a fixed
+ * order (run-to-run deterministic). */
+int b2_trackenv_bins(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
 
 /* Diagnostics (synchronises `cuda_stream`). */
 int b2_stats(b2_sim* sim, void* cuda_stream, B2Stats* out);

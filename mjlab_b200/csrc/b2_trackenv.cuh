@@ -7,7 +7,9 @@
 //          clip (mdp/commands.py:283-352), clip time step + restart of envs that ran off its end -> mask for
 //          b2_forward_masked;
 //   post2 (after the masked forward): anchor-relative body targets (commands.py:354-388), interval push
-//          (events.py:127-143), policy observation with noise and critic observation (:88-150).
+//          (events.py:127-143), policy observation with noise and critic observation (:88-150);
+//   bins (one CTA, between post1 and the forward, motion files only): the adaptive start-frame sampler's EMA and
+//          the CDF post1 inverts (commands.py:256-297, 394-398).
 // The torch implementation in mjlab_b200/envs/tracking_env.py is the reference; both consume the same per-step
 // uniforms U[n][B2_TRACKENV_NU(nu)] (layout in include/b2sim.h), compared in tests.
 #pragma once
@@ -95,6 +97,57 @@ __device__ __forceinline__ void resample(const DevData& dd, const B2TrackEnvArgs
   }
   for (int i = lane; i < 6 * nbody; i += 32) xfrc[i] = 0.f;
 }
+
+// IEEE-rounded division: the library builds with --use_fast_math, but a sampled frame must round as torch's does
+__device__ __forceinline__ float div_rn(float a, float b) {
+#ifdef B2_HOST_EMULATION
+  return a / b;
+#else
+  return __fdiv_rn(a, b);
+#endif
+}
+
+// start frame of a reset or clip restart from its uniform u (B2_START_*, include/b2sim.h)
+__device__ __forceinline__ long long start_frame(const B2TrackEnvArgs& A, float u) {
+  if (A.adaptive == B2_START_FIRST) return 0;
+  if (A.adaptive != B2_START_ADAPTIVE) return (long long)(u * (float)(A.T - 1));
+  int lo = 0, hi = A.nbins - 1;  // first bin with cdf > u (cdf[nbins - 1] = 1 > u)
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (A.cdf[mid] > u) hi = mid; else lo = mid + 1;
+  }
+  const float c0 = lo > 0 ? A.cdf[lo - 1] : 0.f;
+  const float frac = div_rn(u - c0, A.cdf[lo] - c0);
+  const long long ts = (long long)(div_rn((float)lo + frac, (float)A.nbins) * (float)(A.T - 1));
+  return ts < A.T - 1 ? ts : A.T - 1;
+}
+
+// unnormalised start-bin weight: replicate-padded correlation of (EMA + ratio / nbins) with the kernel
+__device__ __forceinline__ float bin_weight(const B2TrackEnvArgs& A, int b, float floor_) {
+  float s = 0.f;
+  for (int i = 0; i < A.adaptive_kernel_size; i++) s += A.adaptive_kernel[i] * (A.bin_fail_ema[min(b + i, A.nbins - 1)] + floor_);
+  return s;
+}
+
+constexpr int kBinThreads = 256;
+
+// sum over the CTA in a fixed order (every thread gets it)
+__device__ __forceinline__ float cta_sum(float v, float* red) {
+  v = wsum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float t = 0.f;
+  for (int k = 0; k < kBinThreads / 32; k++) t += red[k];
+  __syncthreads();
+  return t;
+}
+
+// sum of the bin weights over all bins, block-strided, in a fixed order
+__device__ __forceinline__ float weight_total(const B2TrackEnvArgs& A, float floor_, float* red) {
+  float t = 0.f;
+  for (int b = threadIdx.x; b < A.nbins; b += kBinThreads) t += bin_weight(A, b, floor_);
+  return cta_sum(t, red);
+}
 }  // namespace b2t
 
 __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackEnvArgs A) {
@@ -173,9 +226,14 @@ __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackE
     A.log_row[3 * (size_t)w + 2] = trunc ? 1.f : 0.f;
   }
   for (int a = lane; a < nu; a += 32) last[a] = done ? 0.f : act[a];
+  // a failure counts in the bin of the frame the env reached (commands.py:257-265); time-outs and restarts do not
+  if (A.adaptive == B2_START_ADAPTIVE && term && lane == 0) {
+    const long long bin = ts * A.nbins / A.T;
+    atomicAdd(A.bin_fail_cur + (bin < A.nbins - 1 ? bin : A.nbins - 1), 1.f);
+  }
   // reset onto the clip (RSI), then the clip's time step; envs that ran off its end restart on it
   if (done) {
-    ts = (long long)(U[0] * (float)(A.T - 1));
+    ts = start_frame(A, U[0]);
     resample(dd, A, w, lane, nu, nbody, ts, U);
     ep = 0;
   }
@@ -183,7 +241,7 @@ __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackE
   const bool ended = ts >= A.T;
   if (ended) {
     __syncwarp();
-    ts = (long long)(U[S] * (float)(A.T - 1));
+    ts = start_frame(A, U[S]);
     resample(dd, A, w, lane, nu, nbody, ts, U + S);
   }
   if (lane == 0) {
@@ -281,5 +339,66 @@ __global__ void b2_trackenv_post2_kernel(DevData dd, int nu, int nbody, B2TrackE
     rot6(qmul(qinv(r_quat), quat), ob);
     cr[cb + 3 * b] = pb.x; cr[cb + 3 * b + 1] = pb.y; cr[cb + 3 * b + 2] = pb.z;
     for (int k = 0; k < 6; k++) cr[cb + 3 * A.nb + 6 * b + k] = ob[k];
+  }
+}
+
+// Adaptive start-frame sampler (commands.py:256-297, EMA :394-398), one CTA of kBinThreads between post1 and the
+// masked forward: (1) metrics of the distribution post1 drew from, i.e. the one of the EMA before this step's
+// update; (2) EMA update, this step's counts cleared; (3) CDF of the next step's distribution.  Any nbins: every
+// pass loops over the bins, and the prefix sum walks contiguous per-thread chunks in a fixed order.
+__global__ void __launch_bounds__(b2t::kBinThreads) b2_trackenv_bins_kernel(B2TrackEnvArgs A) {
+  using namespace b2t;
+  __shared__ float red[kBinThreads / 32];
+  __shared__ int redi[kBinThreads / 32];
+  const int t = threadIdx.x, lane = t & 31, nbins = A.nbins;
+  const float floor_ = A.adaptive_uniform_ratio / (float)nbins;
+  // (1) normalised entropy and top-1 bin (first index among equal maxima, as torch.max)
+  float tot = weight_total(A, floor_, red);
+  float h = 0.f, best = -1.f;
+  int besti = 0;
+  for (int b = t; b < nbins; b += kBinThreads) {
+    const float p = div_rn(bin_weight(A, b, floor_), tot);
+    h -= p * (float)log((double)(p + 1e-12f));  // (double: logf is approximate under --use_fast_math)
+    if (p > best) { best = p; besti = b; }
+  }
+  h = cta_sum(h, red);
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+    if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
+  }
+  if (lane == 0) { red[t >> 5] = best; redi[t >> 5] = besti; }
+  __syncthreads();
+  if (t == 0) {
+    for (int k = 1; k < kBinThreads / 32; k++)
+      if (red[k] > best || (red[k] == best && redi[k] < besti)) { best = red[k]; besti = redi[k]; }
+    A.metrics[0] = nbins > 1 ? h / logf((float)nbins) : 1.f;  // one bin: the uniform distribution over the clip
+    A.metrics[1] = best;
+    A.metrics[2] = (float)besti / (float)nbins;
+  }
+  __syncthreads();
+  // (2) EMA of the failure counts
+  for (int b = t; b < nbins; b += kBinThreads) {
+    A.bin_fail_ema[b] = A.adaptive_alpha * A.bin_fail_cur[b] + (1.f - A.adaptive_alpha) * A.bin_fail_ema[b];
+    A.bin_fail_cur[b] = 0.f;
+  }
+  __syncthreads();
+  // (3) CDF: exclusive scan of the per-thread chunk sums, then each chunk in order
+  tot = weight_total(A, floor_, red);
+  const int chunk = (nbins + kBinThreads - 1) / kBinThreads, b0 = min(t * chunk, nbins), b1 = min(b0 + chunk, nbins);
+  float own = 0.f;
+  for (int b = b0; b < b1; b++) own += div_rn(bin_weight(A, b, floor_), tot);
+  float inc = own;
+  for (int o = 1; o < 32; o <<= 1) {
+    const float v = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += v;
+  }
+  if (lane == 31) red[t >> 5] = inc;
+  __syncthreads();
+  float run = inc - own;
+  for (int k = 0; k < (t >> 5); k++) run += red[k];
+  for (int b = b0; b < b1; b++) {
+    run += div_rn(bin_weight(A, b, floor_), tot);
+    A.cdf[b] = b == nbins - 1 ? 1.f : run;  // the last step ends at 1 exactly: every u < 1 finds a bin
   }
 }

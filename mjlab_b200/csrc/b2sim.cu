@@ -1115,6 +1115,12 @@ static int trackenv_check(b2_sim* s, const B2TrackEnvArgs* a) {
       a->root_body < 0 || a->root_body >= s->hm.nbody || a->self_collision_adr < 0 ||
       a->self_collision_adr >= s->hm.nsensordata)
     return fail("b2_trackenv: bad sizes (1 <= nb <= 32 tracked bodies, anchor among them, T >= 2 clip frames)");
+  if (a->adaptive < B2_START_UNIFORM || a->adaptive > B2_START_FIRST)
+    return fail("b2_trackenv: unknown start-frame sampler (adaptive must be one of B2_START_*)");
+  if (a->adaptive == B2_START_ADAPTIVE &&
+      (a->nbins < 1 || a->adaptive_kernel_size < 1 || !a->adaptive_kernel || !a->cdf || !a->bin_fail_ema ||
+       !a->bin_fail_cur || !a->metrics))
+    return fail("b2_trackenv: the adaptive sampler needs nbins >= 1, a kernel of size >= 1 and its five arrays");
   return 0;
 }
 int b2_trackenv_post1(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
@@ -1129,6 +1135,15 @@ int b2_trackenv_post2(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   if (trackenv_check(s, args)) return 1;
   DeviceGuard guard(s->device);
   b2_trackenv_post2_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(s->hd, s->hm.nu, s->hm.nbody, *args);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+int b2_trackenv_bins(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
+  if (trackenv_check(s, args)) return 1;
+  if (args->adaptive != B2_START_ADAPTIVE) return fail("b2_trackenv_bins: the args do not select the adaptive sampler");
+  DeviceGuard guard(s->device);
+  b2_trackenv_bins_kernel<<<1, b2t::kBinThreads, 0, (cudaStream_t)stream>>>(*args);
   s->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -9,11 +9,19 @@ clip (RSI: clip frame + pose / velocity / joint noise, ``mdp/commands.py:283-352
 (``commands.py:354-388``: time step, anchor-relative body targets) -> interval push -> observations (policy
 group with noise, critic group privileged).
 
-The reference needs a motion ``.npz`` from a W&B artifact, which is unavailable offline; the clip here is the
-synthetic one SURVEY.md §8d specifies: the KNEES_BENT pose held for 500 frames (same keys and shapes as
-``commands.py:34-50``, indexed per step exactly like a real clip).  Sampling of the start frame is uniform (the
-adaptive failure-bin sampler of ``commands.py:239-281`` is host-side bookkeeping and, on a static clip, has no
-effect on the physics load).  Everything is mask-based torch code, so one env step is CUDA-graph capturable.
+The clip is ``cfg.motion_file``, a ``.npz`` in the reference's layout (``mjlab_b200.envs.motion``; one can be
+generated with ``tools/make_motion_clip.py``).  Start frames of resets and clip restarts then come from the
+reference's adaptive failure-bin sampler (``commands.py:256-297``, EMA ``:394-398``): the clip is cut into
+``T // (1 / step_dt) + 1`` bins, terminations are counted in the bin of the frame the env reached, their EMA plus a
+uniform floor, smoothed by the kernel ``lambda^i``, is the distribution of the next env step's start bins, and the
+frame is uniform inside the bin.  Each draw inverts that distribution's CDF at the step's own uniform, so the draws
+stay one uniform each; ``sampling_entropy`` / ``sampling_top1_prob`` / ``sampling_top1_bin`` of the distribution
+the step drew from are in its extras.  ``disable_adaptive_sampling`` starts every episode at frame 0.
+
+Without a file the clip is the synthetic one SURVEY.md §8d specifies for the benchmark: the KNEES_BENT pose held
+for ``clip_frames`` frames, start frames uniform (the sampler has no effect on the physics load of a static clip).
+Everything is mask-based torch code (or the fused kernels of ``csrc/b2_trackenv.cuh`` with the sampler's one-CTA
+``b2_trackenv_bins``), so one env step is CUDA-graph capturable.
 """
 
 from __future__ import annotations
@@ -22,9 +30,11 @@ import math
 from dataclasses import dataclass, field
 
 import torch
+import torch.nn.functional as F
 
 from mjlab_b200.asset_zoo import g1, load_compiled
 from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply, quat_apply_inverse, quat_mul
+from mjlab_b200.envs.motion import MotionClip
 from mjlab_b200.envs.velocity_env import _resolve
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg, native
 
@@ -41,12 +51,18 @@ class TrackingEnvCfg:
   num_envs: int = 4096
   decimation: int = 4                 # tracking_env_cfg.py:305
   episode_length_s: float = 10.0      # :306
-  clip_frames: int = 500              # synthetic static clip (SURVEY.md §8d config C)
+  clip_frames: int = 500              # synthetic static clip (SURVEY.md §8d config C); unused with a motion_file
   push_interval_s: tuple = (1.0, 3.0)
   friction_range: tuple = (0.3, 1.2)
   joint_position_range: tuple = (-0.1, 0.1)
   env_spacing: float = 2.5
   seed: int = 42
+  motion_file: str | None = None      # reference-layout .npz (mjlab_b200.envs.motion); None: the synthetic clip
+  adaptive_kernel_size: int = 1       # commands.py:429-433
+  adaptive_lambda: float = 0.8
+  adaptive_uniform_ratio: float = 0.1
+  adaptive_alpha: float = 0.001
+  disable_adaptive_sampling: bool = False
   sim: SimulationCfg = field(
     default_factory=lambda: SimulationCfg(
       nconmax=150_000, njmax=250, mujoco=MujocoCfg(timestep=0.005, iterations=10, ls_iterations=20)))  # :283-291
@@ -122,16 +138,24 @@ class TrackingFlatEnv:
     feet = torch.tensor([m.names["geom"].index(f"robot/{g}") for g in g1.FOOT_GEOMS], device=dev)
     lo, hi = cfg.friction_range
     self.sim.model.geom_friction[:, feet, 0] = self._rand(n, len(feet)) * (hi - lo) + lo
-    # ---- synthetic clip: the keyframe held static (keys of commands.py:34-50) --------------------------
     self.sim.data.qpos[:] = self.default_qpos
     self.sim.data.qvel[:] = 0.0
     self.sim.forward()
-    T, nbk = cfg.clip_frames, len(BODY_NAMES)
-    pose0 = self.robot.body_link_pose_w[0:1, self.body_idx].clone()  # (1, 14, 7) at the world origin
-    self.motion = dict(
-      joint_pos=self.default_joint_pos.expand(T, -1).contiguous(), joint_vel=torch.zeros(T, self.nu, **f32),
-      body_pos_w=pose0[:, :, 0:3].expand(T, -1, -1).contiguous(), body_quat_w=pose0[:, :, 3:7].expand(T, -1, -1).contiguous(),
-      body_lin_vel_w=torch.zeros(T, nbk, 3, **f32), body_ang_vel_w=torch.zeros(T, nbk, 3, **f32))
+    nbk = len(BODY_NAMES)
+    if cfg.motion_file is None:  # synthetic clip: the keyframe held static (keys of commands.py:34-50)
+      T = cfg.clip_frames
+      pose0 = self.robot.body_link_pose_w[0:1, self.body_idx].clone()  # (1, 14, 7) at the world origin
+      self.motion = dict(
+        joint_pos=self.default_joint_pos.expand(T, -1).contiguous(), joint_vel=torch.zeros(T, self.nu, **f32),
+        body_pos_w=pose0[:, :, 0:3].expand(T, -1, -1).contiguous(), body_quat_w=pose0[:, :, 3:7].expand(T, -1, -1).contiguous(),
+        body_lin_vel_w=torch.zeros(T, nbk, 3, **f32), body_ang_vel_w=torch.zeros(T, nbk, 3, **f32))
+      self.start_mode = native.START_UNIFORM
+    else:
+      self.motion = MotionClip.load(cfg.motion_file, ix, BODY_NAMES, self.step_dt, dev).as_dict()
+      T = self.motion["joint_pos"].shape[0]
+      self.start_mode = native.START_FIRST if cfg.disable_adaptive_sampling else native.START_ADAPTIVE
+    self.T = T
+    self._sampler_setup()
     self.time_steps = torch.zeros(n, dtype=torch.long, device=dev)
     self.episode_length_buf = torch.zeros(n, dtype=torch.int32, device=dev)
     self.last_action = torch.zeros(n, self.nu, **f32)
@@ -154,12 +178,68 @@ class TrackingFlatEnv:
   def _clip(self, name):
     return self.motion[name][self.time_steps]
 
+  # -- adaptive start-frame sampler (commands.py:99-110, 256-297, 394-398) -------------------------------
+  def _sampler_setup(self) -> None:
+    cfg, dev = self.cfg, torch.device(self.device)
+    B = self.bin_count = int(self.T // (1 / self.step_dt)) + 1
+    if self.start_mode != native.START_ADAPTIVE:
+      return
+    if cfg.adaptive_kernel_size < 1 or not cfg.adaptive_lambda > 0 or not cfg.adaptive_uniform_ratio > 0 \
+       or not 0.0 <= cfg.adaptive_alpha <= 1.0:
+      raise ValueError("adaptive sampling needs adaptive_kernel_size >= 1, adaptive_lambda > 0, "
+                       "adaptive_uniform_ratio > 0 and 0 <= adaptive_alpha <= 1")
+    k = torch.tensor([cfg.adaptive_lambda**i for i in range(cfg.adaptive_kernel_size)], device=dev)
+    self._bin_kernel = k / k.sum()
+    self.bin_failed_count = torch.zeros(B, device=dev)   # EMA of terminations per bin
+    self._bin_failed_cur = torch.zeros(B, device=dev)    # terminations per bin in the current env step
+    self._metrics = torch.zeros(3, device=dev)            # entropy, top-1 prob, top-1 bin of the last step's draws
+    self._cdf = self._start_distribution()[1].contiguous()  # CDF the next draws invert
+
+  def _start_distribution(self):
+    """(p, CDF) of the start bins from the failure EMA; the CDF's last entry is 1 so that every u < 1 finds a bin."""
+    cfg, B = self.cfg, self.bin_count
+    p = (self.bin_failed_count + cfg.adaptive_uniform_ratio / float(B)).view(1, 1, -1)
+    p = F.conv1d(F.pad(p, (0, cfg.adaptive_kernel_size - 1), mode="replicate"), self._bin_kernel.view(1, 1, -1)).view(-1)
+    p = p / p.sum()
+    cdf = p.cumsum(0)
+    cdf[-1] = 1.0
+    return p, cdf
+
+  def _start_frames(self, u: torch.Tensor) -> torch.Tensor:
+    """Start frame of each env for its uniform ``u`` (B2_START_* of include/b2sim.h)."""
+    T = self.T
+    if self.start_mode == native.START_FIRST:
+      return torch.zeros_like(u, dtype=torch.long)
+    if self.start_mode == native.START_UNIFORM:
+      return (u * (T - 1)).long()
+    B, cdf = self.bin_count, self._cdf
+    b = torch.searchsorted(cdf, u.contiguous(), right=True).clamp_(max=B - 1)  # first bin with cdf > u
+    c0 = torch.where(b > 0, cdf[(b - 1).clamp(min=0)], torch.zeros_like(u))
+    frac = (u - c0) / (cdf[b] - c0)
+    return ((b + frac) / B * (T - 1)).long().clamp_(max=T - 1)
+
+  def _sampler_step(self) -> None:
+    """End of an env step: metrics of the distribution the step drew from, EMA update, CDF for the next step."""
+    B, a = self.bin_count, self.cfg.adaptive_alpha
+    p, _ = self._start_distribution()
+    H = -(p * (p + 1e-12).log()).sum()
+    pmax, imax = p.max(dim=0)
+    self._metrics.copy_(torch.stack([H / math.log(B) if B > 1 else torch.ones_like(H), pmax, imax.float() / B]))
+    self.bin_failed_count.copy_(a * self._bin_failed_cur + (1 - a) * self.bin_failed_count)
+    self._bin_failed_cur.zero_()
+    self._cdf.copy_(self._start_distribution()[1])
+
+  def _extras(self, critic):
+    x = {"critic": critic}
+    if self.start_mode == native.START_ADAPTIVE:
+      x.update(sampling_entropy=self._metrics[0], sampling_top1_prob=self._metrics[1], sampling_top1_bin=self._metrics[2])
+    return x
+
   def _resample(self, mask: torch.Tensor, restart_clip: torch.Tensor, Ub: torch.Tensor) -> None:
     """``MotionCommand._resample_command`` for the masked envs: new clip frame, RSI noise, state write.  ``Ub``:
     this call's uniforms ``[n, 13 + nu]`` (0 clip frame, 1-6 pose, 7-12 velocity, 13.. joints; include/b2sim.h)."""
     n, d = self.num_envs, self.sim.data
-    T = self.cfg.clip_frames
-    ts = (Ub[:, 0] * (T - 1)).long()
+    ts = self._start_frames(Ub[:, 0])
     self.time_steps.copy_(torch.where(restart_clip, ts, self.time_steps))
     pose_n = Ub[:, 1:7] * (self._pr[:, 1] - self._pr[:, 0]) + self._pr[:, 0]
     vel_n = Ub[:, 7:13] * (self._vr[:, 1] - self._vr[:, 0]) + self._vr[:, 0]
@@ -302,10 +382,20 @@ class TrackingFlatEnv:
     A.step_dt = self.step_dt
     A.jp_lo, A.jp_hi = self.cfg.joint_position_range
     A.push_lo, A.push_hi = self.cfg.push_interval_s
-    A.nb, A.nee, A.anchor, A.T = nb, len(EE_NAMES), self.anchor, self.cfg.clip_frames
+    A.nb, A.nee, A.anchor, A.T = nb, len(EE_NAMES), self.anchor, self.T
     A.self_collision_adr = self.self_collision_adr[0]
     A.root_body = int(self.robot.indexing.root_body_id)
     A.max_episode_length = self.max_episode_length
+    A.adaptive = self.start_mode
+    if self.start_mode == native.START_ADAPTIVE:
+      sampler = dict(adaptive_kernel=self._bin_kernel, cdf=self._cdf, bin_fail_ema=self.bin_failed_count,
+                     bin_fail_cur=self._bin_failed_cur, metrics=self._metrics)
+      for k, t in sampler.items():
+        assert t.is_contiguous() and t.dtype == torch.float32, k
+        setattr(A, k, t.data_ptr())
+      ptr.update(sampler)
+      A.adaptive_alpha, A.adaptive_uniform_ratio = self.cfg.adaptive_alpha, self.cfg.adaptive_uniform_ratio
+      A.nbins, A.adaptive_kernel_size = self.bin_count, self.cfg.adaptive_kernel_size
     self._native_args = A
     self._keep = ptr
 
@@ -324,9 +414,11 @@ class TrackingFlatEnv:
                                         ctypes.c_void_p(self.action_scale.data_ptr()), st))
     sim.step_n(self.cfg.decimation)
     native.check(sim._lib.b2_trackenv_post1(sim._h, ctypes.byref(self._native_args), st))
+    if self.start_mode == native.START_ADAPTIVE:
+      native.check(sim._lib.b2_trackenv_bins(sim._h, ctypes.byref(self._native_args), st))
     sim.forward(env_mask=self._done_buf)
     native.check(sim._lib.b2_trackenv_post2(sim._h, ctypes.byref(self._native_args), st))
-    return self._obs, self._reward, self._term, self._trunc, {"critic": self._critic}
+    return self._obs, self._reward, self._term, self._trunc, self._extras(self._critic)
 
   def _step_torch(self, action: torch.Tensor, U: torch.Tensor):
     cfg, d, n, nu = self.cfg, self.sim.data, self.num_envs, self.nu
@@ -345,6 +437,9 @@ class TrackingFlatEnv:
     bad_ori = (quat_apply_inverse(a_quat, g)[:, 2] - quat_apply_inverse(r_quat, g)[:, 2]).abs() > 0.8
     ee_err = (self.body_pos_relative_w[:, self.ee_idx, 2] - pos[:, self.ee_idx, 2]).abs()
     terminated = bad_z | bad_ori | (ee_err > 0.25).any(dim=1)
+    if self.start_mode == native.START_ADAPTIVE:  # failures, in the bin of the frame reached (commands.py:257-265)
+      fail_bin = (self.time_steps * self.bin_count // self.T).clamp_(0, self.bin_count - 1)
+      self._bin_failed_cur.index_add_(0, fail_bin, terminated.float())
     # rewards (:200-250)
     r = 0.5 * torch.exp(-((a_pos - r_pos) ** 2).sum(-1) / 0.3**2)
     r = r + 0.5 * torch.exp(-quat_error_magnitude(a_quat, r_quat) ** 2 / 0.4**2)
@@ -366,8 +461,10 @@ class TrackingFlatEnv:
     self.episode_length_buf.copy_(torch.where(done, torch.zeros_like(self.episode_length_buf), self.episode_length_buf))
     self.last_action.copy_(torch.where(done.unsqueeze(1), torch.zeros_like(self.last_action), self.last_action))
     self.time_steps += 1
-    ended = self.time_steps >= cfg.clip_frames
+    ended = self.time_steps >= self.T
     self._resample(ended, ended, U[:, S:2 * S])
+    if self.start_mode == native.START_ADAPTIVE:
+      self._sampler_step()
     self._done_buf.copy_(done | ended)
     self.sim.forward(env_mask=self._done_buf)
     self._update_command()
@@ -381,7 +478,7 @@ class TrackingFlatEnv:
     lo_t, hi_t = cfg.push_interval_s
     self.push_time_left.copy_(torch.where(push, P[:, 6] * (hi_t - lo_t) + lo_t, self.push_time_left))
     policy, critic = self.observations(U[:, 2 * S + 7:])
-    return policy, reward, terminated, truncated, {"critic": critic}
+    return policy, reward, terminated, truncated, self._extras(critic)
 
   def close(self):
     self.sim.close()

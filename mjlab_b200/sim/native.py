@@ -65,7 +65,13 @@ class B2TrackEnvArgs(ctypes.Structure):
     + [("pose_range", ctypes.c_float * 12), ("vel_range", ctypes.c_float * 12)]
     + [(n, ctypes.c_float) for n in ("step_dt", "jp_lo", "jp_hi", "push_lo", "push_hi")]
     + [(n, ctypes.c_int32) for n in ("nb", "nee", "anchor", "T", "self_collision_adr", "root_body", "max_episode_length")]
+    + [(n, ctypes.c_void_p) for n in ("adaptive_kernel", "cdf", "bin_fail_ema", "bin_fail_cur", "metrics")]
+    + [(n, ctypes.c_float) for n in ("adaptive_alpha", "adaptive_uniform_ratio")]
+    + [(n, ctypes.c_int32) for n in ("nbins", "adaptive", "adaptive_kernel_size")]
   )
+
+
+START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
 
 
 def make_model_desc(model):
@@ -122,6 +128,7 @@ def bind(L: ctypes.CDLL) -> ctypes.CDLL:
     "b2_velenv_post": ([vp, P(B2VelEnvArgs), vp], ci),
     "b2_trackenv_post1": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_trackenv_post2": ([vp, P(B2TrackEnvArgs), vp], ci),
+    "b2_trackenv_bins": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_stats": ([vp, vp, P(B2Stats)], ci),
     "b2_launch_count": ([vp], ctypes.c_int64),
     "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),

@@ -22,3 +22,19 @@ for _ in range(12):
   trk.step(torch.rand((n, trk.nu), generator=g, device="cuda:0") * 2 - 1)
 torch.cuda.synchronize()
 print("tracking env ok")
+# a moving clip with the adaptive start-frame sampler (b2_trackenv_bins), falls forced so that failures are binned
+sys.path.insert(0, str(Path(__file__).resolve().parent))
+import tempfile  # noqa: E402
+
+from make_motion_clip import make_clip  # noqa: E402
+
+with tempfile.TemporaryDirectory() as tmp:
+  clip = make_clip(Path(tmp) / "clip.npz", frames=960, device="cuda:0")
+  ad = TrackingFlatEnv(TrackingEnvCfg(num_envs=n, motion_file=clip, adaptive_kernel_size=3), device="cuda:0")
+  for k in range(12):
+    if k % 3 == 0:
+      ad.sim.data.qpos[: n // 4, 2] -= 0.4
+    ad.step(torch.rand((n, ad.nu), generator=g, device="cuda:0") * 2 - 1)
+  torch.cuda.synchronize()
+  assert float(ad.bin_failed_count.sum()) > 0
+  print("adaptive tracking env ok")
