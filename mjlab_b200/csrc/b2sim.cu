@@ -112,6 +112,25 @@ __global__ void b2_static_rows_kernel(float* xpos, int xpos_stride, float* xmat,
   for (int i = 0; i < 9; i++) xmat[w * xmat_stride + 9 * g + i] = p[3 + i];
 }
 
+// The float part of the compact kinematic records (kinematic_tables), rebuilt from the shared rows of body_pos,
+// body_quat, jnt_pos, jnt_axis and qpos0, so that a caller's write to one of them reaches the fast kinematics.  Only
+// launched while the records are in use (fastkin: none of the five fields is expanded); the int words stay as built.
+// (The joint and qpos address come from the records' own int words: two dependent loads per body, not four.)
+__global__ void b2_kinrec_kernel(DevModel m) {
+  float* rec = (float*)m.kinrec;
+  for (int b = threadIdx.x; b < m.nbody; b += blockDim.x) {
+    float* r = rec + 16 * b;
+    const int tj = __float_as_int(r[11]), qa = __float_as_int(r[15]);
+    for (int k = 0; k < 3; k++) r[k] = m.body_pos.p[3 * b + k];
+    for (int k = 0; k < 4; k++) r[4 + k] = m.body_quat.p[4 * b + k];
+    if ((tj & 0xff) != 0xff) {
+      const int j = tj >> 8;
+      for (int k = 0; k < 3; k++) { r[8 + k] = m.jnt_pos.p[3 * j + k]; r[12 + k] = m.jnt_axis.p[3 * j + k]; }
+      r[3] = m.qpos0.p[qa];
+    }
+  }
+}
+
 // Heavy-first dispatch: order worlds by the previous step's (Newton iterations, contacts),
 // descending, with a one-CTA counting sort (128 buckets).  Only scheduling changes, not results.
 // Key = (Newton iterations, solver block class, contacts / 8): under phase-synchronous execution the warps of a
@@ -314,6 +333,16 @@ static int add_data(b2_sim* s, const DataArray<A>& r) {
   a.p = (T*)p; a.stride = stride; a.n = r.n;
   s->data_fields.push_back(make_field(r.name, p, std::is_same<T, int>::value ? B2_I32 : B2_F32, s->nworld, stride, r.n,
                                       r.width, r.per_world));
+  return 0;
+}
+
+// Every entry that launches the step kernel calls this first, on the caller's stream (before any partition fork, so
+// that a captured graph holds it).
+static int refresh_kinrec(b2_sim* s, cudaStream_t st) {
+  if (!s->hm.fastkin) return 0;
+  b2_kinrec_kernel<<<1, 64, 0, st>>>(s->hm);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
@@ -963,7 +992,7 @@ int b2_expand_model_field(b2_sim* s, const char* name, void* stream, B2Tensor* o
     const DevModel& m = s->hm;
     if (f->farr == &m.body_pos || f->farr == &m.body_quat || f->farr == &m.jnt_pos || f->farr == &m.jnt_axis ||
         f->farr == &m.qpos0)
-      s->hm.fastkin = 0;  // the compact kinematic records mirror the shared arrays only
+      s->hm.fastkin = 0;  // the compact kinematic records hold one row: per-world frames take the generic walk
     f->ptr = p; f->stride[0] = n;
   }
   if (out) fill_tensor(s, *f, out);
@@ -1038,16 +1067,17 @@ int b2_get_option(b2_sim* s, const char* key, double* v) {
 int b2_step(b2_sim* s, void* stream) {
   if (!s) return fail("b2_step: null sim");
   DeviceGuard guard(s->device);
-  return launch(s, true, (cudaStream_t)stream);
+  return refresh_kinrec(s, (cudaStream_t)stream) || launch(s, true, (cudaStream_t)stream);
 }
 int b2_forward(b2_sim* s, void* stream) {
   if (!s) return fail("b2_forward: null sim");
   DeviceGuard guard(s->device);
-  return launch(s, false, (cudaStream_t)stream);
+  return refresh_kinrec(s, (cudaStream_t)stream) || launch(s, false, (cudaStream_t)stream);
 }
 int b2_forward_masked(b2_sim* s, const unsigned char* world_mask_dev, void* stream) {
   if (!s) return fail("b2_forward_masked: null sim");
   DeviceGuard guard(s->device);
+  if (refresh_kinrec(s, (cudaStream_t)stream)) return 1;
   s->hd.world_mask = world_mask_dev;
   int rc = launch(s, false, (cudaStream_t)stream);
   s->hd.world_mask = nullptr;
@@ -1058,6 +1088,7 @@ int b2_step_n(b2_sim* s, int n, void* stream) {
   DeviceGuard guard(s->device);
   if (n <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
+  if (refresh_kinrec(s, st)) return 1;
   if (s->fused_decimation) return launch(s, true, st, n);
   int np = std::min(std::max(s->split_streams, 1), 4);
   if (np > 1 && n > 1 && s->nworld >= 1024 * np) {
