@@ -207,6 +207,16 @@ __device__ __forceinline__ float b2_rcp(float x) {
   return r;
 #endif
 }
+// The same value, but one the compiler may not merge with other reads of it.  The kernel forms its region
+// pointers as s + fresh(L.<region>) where it uses them: the offset is a constant-bank operand and the pointer one
+// add, whereas a pointer formed once per environment is held in a register (two, as a call argument) through
+// every phase in between, which at 128 registers per thread means spilling it.
+__device__ __forceinline__ int fresh(int v) {
+#ifndef B2_HOST_EMULATION
+  asm volatile("mov.b32 %0, %0;" : "+r"(v));
+#endif
+  return v;
+}
 // ---- bottom-up blocked L^T D L (leaves first) -----------------------------------------------------------
 // Pivots are eliminated from the last dof to the first, four per block step, so the dof tree's zero pattern
 // survives (no fill between branches) and the trailing update visits only the entries the tree can make
@@ -922,7 +932,7 @@ __device__ __noinline__ float rows_cost(int fc, int fl, const float* con, const 
 // convex routines are ~120 KB of code: models without such pairs (BASELINE configs A-E) run the instantiation
 // that does not contain them (their presence alone would weigh on the G1 step through code layout).
 template <int MODE>
-__global__ void __launch_bounds__(32 * B2_WARPS_PER_CTA, B2_MIN_CTAS)
+__global__ void __launch_bounds__(32 * B2_WARPS_PER_CTA, (MODE & 2) ? B2_MIN_CTAS_CVX : B2_MIN_CTAS)
 b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevData dd) {
   using namespace b2;
   constexpr bool STEP = (MODE & 1) != 0, CVX = (MODE & 2) != 0;
@@ -936,8 +946,8 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   // per-CTA copy of the factorisation pair schedule (shared by the CTA's warps)
   unsigned* s_sched = (unsigned*)(smem_all + (size_t)B2_WARPS_PER_CTA * m.lay.total);
 #define SCHED s_sched, (const int*)s_sched + m.ldl_nsparse, m.ldl_dense
-#define FACTOR(sp) ldl_factor(H, invdiag, nv, SCHED, sp, lane)
-#define SOLVE(v, tree) ldl_solve(H, invdiag, v, nv, lane)
+#define FACTOR(sp) ldl_factor(BLK(H), BLK(invdiag), nv, SCHED, sp, lane)
+#define SOLVE(v, tree) ldl_solve(BLK(H), BLK(invdiag), v, nv, lane)
   // Phase-synchronous execution (dd.phase_sync): the kernel's code is ~200 KB against a 32 KB instruction cache,
   // so the CTA's warps are re-aligned at every phase boundary and they fetch the same code together.
   // Levels: 1 = major phases + one vote per Newton iteration, 2 = + the three segments of an iteration,
@@ -976,12 +986,40 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   long long tphase_ = clock64();
 #endif
 
-  // ---------------- phase 0: TMA bulk load of this environment's state -------------------------
-  float* qpos = s + L.qpos; float* qvel = s + L.qvel; float* qacc_ws = s + L.qacc_ws;
+  // Regions of this environment's shared-memory block and its rows of global arrays.  REGIONS() forms them anew at
+  // the start of every phase (s + offset, offsets from the constant bank): a pointer then lives through the phase
+  // that uses it, not through the whole step, and the pointers that do not appear in a phase cost nothing there.
+  // The arguments of the out-of-line helpers are formed at the call (BLK) for the same reason.
+#define BLK(region) (s + fresh(L.region))
+#define ROW(field) (dd.field.p + (size_t)w * fresh(dd.field.stride))
+#define REGIONS()                                                                                      \
+  do {                                                                                                 \
+    qpos = BLK(qpos); qvel = BLK(qvel); qacc_ws = BLK(qacc_ws);                                        \
+    ctrl = ROW(ctrl); qfrc_applied = ROW(qfrc_applied); xfrc = ROW(xfrc_applied); Mq = ROW(qM_packed); \
+    xpos = BLK(xpos); xquat = BLK(xquat); xipos = BLK(xipos);                                          \
+    scom = BLK(scom); xanchor = BLK(xanchor); xaxis = BLK(xaxis);                                      \
+    cinert = BLK(cinert); crb = BLK(crb); cdof = BLK(cdof);                                            \
+    cdofdot = BLK(cdofdot); cvel = BLK(cvel); cacc = BLK(cacc);                                        \
+    H = BLK(H); invdiag = BLK(invdiag);                                                                \
+    qfrc_smooth = BLK(qfrc_smooth); qacc_smooth = BLK(qacc_smooth);                                    \
+    qacc = BLK(qacc); Ma = BLK(Ma); grad = BLK(grad);                                                  \
+    Mv = BLK(Mv); qfrc_c = BLK(qfrc_c); tmpv = BLK(tmpv); actf = BLK(actf);                            \
+    gpose = BLK(gpose); con = BLK(contacts); lim = BLK(limits); gstart = (int*)BLK(gstart);            \
+    gV = BLK(gV); Mred = BLK(Mred);                                                                    \
+    gA = BLK(gA); gu = BLK(gu); glist = (int*)BLK(glist); gW = BLK(gW);                                \
+  } while (0)
+  float *qpos, *qvel, *qacc_ws;
   // inputs with a single use (phase 4) are read from global memory in place
-  const float* ctrl = dd.ctrl.p + (size_t)w * dd.ctrl.stride;
-  const float* qfrc_applied = dd.qfrc_applied.p + (size_t)w * dd.qfrc_applied.stride;
-  const float* xfrc = dd.xfrc_applied.p + (size_t)w * dd.xfrc_applied.stride;
+  const float *ctrl, *qfrc_applied, *xfrc;
+  float *xpos, *xquat, *xipos, *scom, *xanchor, *xaxis, *cinert, *crb, *cdof, *cdofdot, *cvel, *cacc;
+  float *H, *invdiag;
+  // the joint-space inertia lives in global memory (2.5 KB per env, L2-resident): it is written once, copied
+  // into H before each factorisation and read by symv only when the solver runs on all dofs
+  float* Mq;
+  float *qfrc_smooth, *qacc_smooth, *qacc, *Ma, *grad, *Mv, *qfrc_c, *tmpv, *actf;
+  float *gpose, *con, *lim, *gV, *Mred, *gA, *gu, *gW;  // (collision and constraints overlay the smooth-only regions)
+  int *gstart, *glist;
+  REGIONS();
   {
     unsigned long long* bar = &bars[warp];
     fence_async_smem();  // the previous environment's generic-proxy accesses precede this one's bulk writes
@@ -1000,18 +1038,6 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(0);
   PSYNC();
-  float* xpos = s + L.xpos; float* xquat = s + L.xquat; float* xipos = s + L.xipos;
-  float* scom = s + L.scom; float* xanchor = s + L.xanchor; float* xaxis = s + L.xaxis;
-  float* cinert = s + L.cinert; float* crb = s + L.crb; float* cdof = s + L.cdof;
-  float* cdofdot = s + L.cdofdot; float* cvel = s + L.cvel; float* cacc = s + L.cacc;
-  float* H = s + L.H; float* invdiag = s + L.invdiag;
-  // the joint-space inertia lives in global memory (2.5 KB per env, L2-resident): it is written once, copied
-  // into H before each factorisation and read by symv only when the solver runs on all dofs
-  float* Mq = dd.qM_packed.p + (size_t)w * dd.qM_packed.stride;
-  float* qfrc_smooth = s + L.qfrc_smooth; float* qacc_smooth = s + L.qacc_smooth;
-  float* qacc = s + L.qacc; float* Ma = s + L.Ma; float* grad = s + L.grad;
-  float* Mv = s + L.Mv; float* qfrc_c = s + L.qfrc_c;
-  float* tmpv = s + L.tmpv; float* actf = s + L.actf;
 
   // The decimation loop (manager_based_rl_env.py:109-114: ctrl held, `decimation` x sim.step) runs inside
   // the launch: state vectors stay in shared memory between sub-steps.
@@ -1023,6 +1049,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   const bool emit = dd.emit != 0 && lastsub;
   bool ctrl_changed = false;
   // ---------------- phase 1: kinematics (lane per body, private walk down its ancestor chain) ----
+  REGIONS();
   {
     const float* body_pos = MP(body_pos); const float* body_quat = MP(body_quat);
     const float* jnt_pos = MP(jnt_pos); const float* jnt_axis = MP(jnt_axis);
@@ -1154,8 +1181,8 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(1);
   PSYNC();
+  REGIONS();
   // geom / site world poses -> global (and shared for collidable geoms)
-  float* gpose = s + L.gpose;
   {
     const float* geom_pos = MP(geom_pos); const float* geom_quat = MP(geom_quat);
     const float* geom_rb = MP(geom_rbound); const float* geom_mar = MP(geom_margin);
@@ -1203,6 +1230,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(2);
   PSYNC();
+  REGIONS();
   // ---------------- phase 2: subtree com, spatial inertias, motion vectors -----------------------
   {
     const float* mass = MP(body_mass); const float* sub = MP(body_subtreemass);
@@ -1310,6 +1338,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(3);
   PSYNC();
+  REGIONS();
   // ---------------- phase 3: composite inertias -> joint-space inertia M (packed lower) ----------
   #pragma unroll 1
   for (int b = lane; b < nb; b += 32) {
@@ -1341,6 +1370,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(4);
   PSYNC();
+  REGIONS();
   // ---------------- phase 4: velocities, bias forces, actuation, qfrc_smooth ----------------------
   #pragma unroll 1
   for (int b = lane; b < nb; b += 32) {
@@ -1498,10 +1528,8 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(5);
   PSYNC();
+  REGIONS();
   // ---------------- phase 5: collision (static pair table, bounding-sphere filter, primitives) ----
-  float* con = s + L.contacts;   // overlays the smooth-only regions (cinert, crb, cdofdot, cacc, ...)
-  float* lim = s + L.limits;
-  int* gstart = (int*)(s + L.gstart);
   int ncon = 0, overflow = 0;
   {
     int* pairlist = (int*)(s + L.pairlist);
@@ -1920,6 +1948,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(6);
   PSYNC();
+  REGIONS();
   // ---------------- phase 6: joint-limit rows, body-pair groups ----------------------------------
   int nlim = 0;
   {
@@ -2037,8 +2066,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     nefc += cnt;
   }
 
-  float* gV = s + L.gV;
-#define MULJ(x, dc, dl, acc) mulJ(x, dc, dl, acc, con, lim, gstart, gV, cdof, m.body_dofmask, ncon, nlim, ngroup, MC, NLC, lane)
+#define MULJ(x, dc, dl, acc) mulJ(x, dc, dl, acc, BLK(contacts), BLK(limits), (int*)BLK(gstart), BLK(gV), BLK(cdof), m.body_dofmask, ncon, nlim, ngroup, MC, NLC, lane)
   // CJAR <- -aref = B*vel_row + K*imp*(pos-margin) for contact rows (0 for unused rows)
   if (nefc > 0) {
     MULJ(qvel, CJV0, LJV, false);
@@ -2055,11 +2083,11 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(7);
   PSYNC();
+  REGIONS();
   // ---------------- phase 7: unconstrained acceleration -------------------------------------------
   #pragma unroll 1
   for (int i = lane; i < (m.ntri + 3) >> 2; i += 32) ((float4*)H)[i] = ((const float4*)Mq)[i];  // both rows are 16 B aligned and padded
   __syncwarp();
-  float* Mred = s + L.Mred;
   ldl_factor(H, invdiag, nv, SCHED, true, lane, 0, (reduced && nefc > 0) ? n : 0, Mred);
   SOLVE(qacc_smooth, true);
   if (m.debug & 1)
@@ -2068,13 +2096,13 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(8);
   PSYNC();
+  REGIONS();
   // ---------------- phase 8: Newton solver (primal, exact line search) ----------------------------
   int niter = 0, nls = 0;
   float cost = 0.f;
   const float* Mr = reduced ? Mred : Mq;  // reduced problem: Schur complement of M on the leading block
   const float* qs = qfrc_smooth;
   const float scale = 1.f / (m.meaninertia * (float)max(1, nv));
-  float* gA = s + L.gA; float* gu = s + L.gu; int* glist = (int*)(s + L.glist); float* gW = s + L.gW;
   float oldcost = 0.f;
   bool first = true;
   // Conjugate gradient variant (opt.solver = CG; mujoco_warp's second solver): same cost, same update pass and
@@ -2147,6 +2175,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   #pragma unroll 1
   while (true) {
     if (psync) { if (!__syncthreads_or(run ? 1 : 0)) break; } else if (!run) break;
+    REGIONS();
     if (run) do {
       // ---- constraint update: forces, cost, active set, qfrc_constraint = J^T f ---------------
       float cst = 0.f;
@@ -2265,6 +2294,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     } while (0);
     PHASE_MARK(12);
     PSYNC_L(2);
+    REGIONS();
     if (run && !refine && !cg) {
       // ---- Hessian H = M + J^T D_active J via per-body-pair 6x6 blocks -------------------------
       {  // leading block only: the rows of the eliminated dofs keep the factor of M (needed after the loop)
@@ -2338,6 +2368,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     }
     PHASE_MARK(13);
     PSYNC_L(2);
+    REGIONS();
     if (run && !cg) {
       if (!refine) ldl_factor(H, invdiag, n, SCHED, treeok, lane, (nv - n) >> 2);
       #pragma unroll 1
@@ -2364,6 +2395,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     }
     PHASE_MARK(14);
     PSYNC_L(2);
+    REGIONS();
     if (run) do {
       // ---- exact line search along `search` --------------------------------------------------
       symv(Mr, search, Mv, n, lane);
@@ -2479,6 +2511,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
       niter++;
     } while (0);
   }
+  REGIONS();
   if (nefc > 0) {
     if (reduced) {
       // eliminated dofs: a_c = a_s,c - L_cc^-1 L_cd (a_d - a_s,d), i.e. rows k >= n of L x = 0 with x_d given
@@ -2508,6 +2541,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   }
   PHASE_MARK(9);
   PSYNC();
+  REGIONS();
   // ---------------- phase 9: contact forces, sensors -----------------------------------------------
   {
     float* g_force = dd.contact_force.p + (size_t)w * dd.contact_force.stride;
@@ -2606,6 +2640,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
 
   PHASE_MARK(10);
   PSYNC();
+  REGIONS();
   // ---------------- phase 10: integrate (implicitfast / Euler), write state ------------------------
   float* gq = dd.qpos.p + (size_t)w * dd.qpos.stride;
   float* gv = dd.qvel.p + (size_t)w * dd.qvel.stride;

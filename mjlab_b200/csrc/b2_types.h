@@ -5,12 +5,16 @@
 #ifndef B2_WARPS_PER_CTA
 #define B2_WARPS_PER_CTA 4
 #endif
+// Co-resident CTAs per SM that the step kernel's register budget is cut for (65536 registers per SM).  The kernel
+// forms its region pointers where it uses them (b2_kernel.cuh, REGIONS), so for sm_90a ptxas fits the primitive-only
+// instantiations (<0>, <1>) into 128 registers without spills: 16 warps per SM.  The instantiations with the convex
+// routines (<2>, <3>, models with mesh or height-field pairs) spill a few words at 128 and keep 12 warps per SM
+// (up to 168 registers).  DESIGN.md §4.1 has the measurements.
 #ifndef B2_MIN_CTAS
-// 12 warps per SM (up to 168 registers): for sm_90a, ptxas fits the step kernel into 128 registers (16 warps per SM)
-// only with spills, 0.2 KB of stores and 0.6 KB of loads per thread.  Measured on an H100 at 4096 envs, 12 warps per
-// SM are 8 % faster per sub-step on the G1 flat scene and 6 % on the height-field terrain, and 13 % slower on the Go1
-// box terrain (DESIGN.md §4.1).
-#define B2_MIN_CTAS (12 / B2_WARPS_PER_CTA)
+#define B2_MIN_CTAS (16 / B2_WARPS_PER_CTA)
+#endif
+#ifndef B2_MIN_CTAS_CVX
+#define B2_MIN_CTAS_CVX (12 / B2_WARPS_PER_CTA)
 #endif
 #define B2_MAX_FIELDS 96
 

@@ -876,7 +876,9 @@ static int launch_resources(b2_sim* s) {
   s->tickets = (int*)p;
   cudaMemset(p, 0, sizeof(int) * 4);
   int per_sm = 0, sms = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, b2_step_kernel<1>, 32 * B2_WARPS_PER_CTA, s->smem_bytes);
+  // (of the instantiation that steps this model: the convex one has a larger register budget)
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, s->has_convex ? b2_step_kernel<3> : b2_step_kernel<1>,
+                                                32 * B2_WARPS_PER_CTA, s->smem_bytes);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device);
   s->resident_ctas = per_sm * sms;
   for (int h = 0; h < 4; h++)
