@@ -84,9 +84,13 @@ const char* b2_field_name(b2_sim* sim, int which, int index);
 /* Tile a Model field to a real leading nworld dimension (reference randomization.py:20-55). */
 int b2_expand_model_field(b2_sim* sim, const char* name, void* cuda_stream, B2Tensor* out);
 
-/* Options: "iterations", "ls_iterations", "tolerance", "ls_tolerance", "ls_parallel",
- * "timestep", "integrator", "debug_outputs", "sorted_dispatch" (heavy-first launch order, default on), "fused_decimation" (b2_step_n as one launch; default off),
- * "dense_factor" (testing: always take the dense factorisation schedule instead of the dof-tree one). */
+/* Options, set and read back: "iterations", "ls_iterations", "tolerance", "ls_tolerance", "timestep",
+ * "integrator", "solver" (1 = CG, 2 = Newton), "debug_outputs" (also write qfrc_bias, qfrc_smooth, qM,
+ * qacc_smooth and qfrc_constraint), "sorted_dispatch" (heavy-first launch order, default on),
+ * "dense_factor" (testing: always take the dense factorisation schedule instead of the dof-tree one),
+ * "full_solver" (testing: Newton on all dofs even when a leading block suffices).
+ * Read only: "smem_bytes_per_env", "maxcon", "resident_ctas", "reduced_block_cap".
+ * Any other name is refused as an unknown option. */
 int b2_set_option(b2_sim* sim, const char* key, double value);
 int b2_get_option(b2_sim* sim, const char* key, double* value);
 
@@ -100,9 +104,9 @@ int b2_step_n(b2_sim* sim, int n, void* cuda_stream);     /* n sub-steps with ct
 int b2_forward_masked(b2_sim* sim, const unsigned char* world_mask_dev, void* cuda_stream);
 
 /* End-to-end call with HOST buffers (pinned or pageable): copies `ctrl` (nworld*nu floats, row
- * stride nu) to the device, runs `nsubstep` steps, copies qpos (nworld*nq) and qvel (nworld*nv)
+ * stride nu) to the device, runs `nsteps` sub-steps, copies qpos (nworld*nq) and qvel (nworld*nv)
  * back; asynchronous on `cuda_stream` when the host buffers are pinned. NULL outputs are skipped. */
-int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsubstep, float* qpos_host,
+int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_host,
                  float* qvel_host, void* cuda_stream);
 
 /* Fused MDP glue of the velocity-tracking task around the step (SURVEY.md §8f-1..3): what

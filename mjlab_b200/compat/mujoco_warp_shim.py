@@ -128,7 +128,6 @@ def put_data(mjm, mjd=None, nworld: int = 1, nconmax=None, njmax=None, **_) -> D
   d._bind(eng)
   if m is not None:
     m._bind(eng)
-    eng.lib.b2_set_option(eng.h, b"ls_parallel", float(bool(m.opt.ls_parallel)))
   object.__setattr__(d, "_model", m)
   if mjd is not None and hasattr(mjd, "qpos"):
     import numpy as np

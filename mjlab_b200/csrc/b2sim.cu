@@ -62,16 +62,10 @@ struct b2_sim {
   int64_t launches = 0;
   int* order = nullptr;       // heavy-first dispatch order (device)
   int sorted_dispatch = 1;
-  int fused_decimation = 0;
-  int split_streams = 2;       // b2_step_n runs this many env partitions on internal streams
-  int reorder_every_substep = 1;  // heavy-first order recomputed before every sub-step (fresh Newton counts keep phase-synchronous CTAs balanced)
-  int phase_sync = 2;          // CTA barriers at phase boundaries, level 0..3 (instruction-cache locality)
   int has_convex = 0;          // the model has mesh / height-field collision pairs: kernels with the convex routines
-  int work_queue = 0;          // warps pull environments from a ticket counter (persistent grid)
-  int* tickets = nullptr;      // one counter per stream partition (device)
   int resident_ctas = 0;       // co-resident CTAs of the step kernel on this device
-  cudaStream_t side[4] = {nullptr, nullptr, nullptr, nullptr};
-  cudaEvent_t ev_fork = nullptr, ev_join[4] = {nullptr, nullptr, nullptr, nullptr};  // off by default
+  cudaStream_t side[2] = {nullptr, nullptr};  // b2_step_n's two env partitions
+  cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
   size_t smem_bytes = 0;
 };
 
@@ -140,9 +134,8 @@ __device__ __forceinline__ int b2_order_key(int niter, int nd, int ncon, int nd_
 }
 __global__ void b2_order_kernel(const int* __restrict__ niter, int niter_stride, const int* __restrict__ ncon,
                                 int ncon_stride, const int* __restrict__ nd, int nd_stride, int nd_small,
-                                int base_world, int count, int* __restrict__ order, int* __restrict__ ticket) {
+                                int base_world, int count, int* __restrict__ order) {
   __shared__ int hist[128];
-  if (ticket != nullptr && threadIdx.x == 0) *ticket = 0;  // the step kernel's work queue starts empty
   __shared__ int base[128];
   for (int i = threadIdx.x; i < 128; i += blockDim.x) hist[i] = 0;
   __syncthreads();
@@ -346,33 +339,23 @@ static int refresh_kinrec(b2_sim* s, cudaStream_t st) {
   return 0;
 }
 
-static int launch(b2_sim* s, bool step, cudaStream_t st, int nsub = 1, int base = 0, int count = -1, int part = 0,
-                  int emit = 1, bool reorder = true) {
+static int launch(b2_sim* s, bool step, cudaStream_t st, int base = 0, int count = -1, int emit = 1) {
   if (count < 0) count = s->nworld;
-  s->hd.nsub = nsub;
   s->hd.emit = emit;
   s->hd.world_base = base;
   s->hd.world_count = count;
-  int grid = (count + B2_WARPS_PER_CTA - 1) / B2_WARPS_PER_CTA;
-  const bool queue = s->work_queue && s->tickets && s->resident_ctas > 0 && grid > s->resident_ctas;
-  int* ticket = queue ? s->tickets + part : nullptr;
+  const int grid = (count + B2_WARPS_PER_CTA - 1) / B2_WARPS_PER_CTA;
   if (step && s->sorted_dispatch && s->order && count >= 512 && s->hd.world_mask == nullptr) {
-    // (the order of the first sub-step of a decimation loop serves the whole loop: costs change little within it)
-    if (reorder || queue) {
-      b2_order_kernel<<<1, 1024, 0, st>>>(s->hd.solver_niter.p, s->hd.solver_niter.stride, s->hd.ncon.p,
-                                          s->hd.ncon.stride, s->hd.solver_nd.p, s->hd.solver_nd.stride,
-                                          s->hm.lay.ndcap, base, count, s->order, ticket);
-      s->launches++;
-    }
+    b2_order_kernel<<<1, 1024, 0, st>>>(s->hd.solver_niter.p, s->hd.solver_niter.stride, s->hd.ncon.p,
+                                        s->hd.ncon.stride, s->hd.solver_nd.p, s->hd.solver_nd.stride,
+                                        s->hm.lay.ndcap, base, count, s->order);
+    s->launches++;
     s->hd.world_order = s->order;
   } else {
     s->hd.world_order = nullptr;
-    if (queue) CUDA_OK(cudaMemsetAsync(ticket, 0, sizeof(int), st));
   }
-  s->hd.ticket = ticket;
   // phase-synchronous warps need every warp of every CTA to own an environment (no early exits, no mask)
-  s->hd.phase_sync = (!queue && s->hd.world_mask == nullptr && count % B2_WARPS_PER_CTA == 0) ? s->phase_sync : 0;
-  if (queue) grid = s->resident_ctas;
+  s->hd.phase_sync = s->hd.world_mask == nullptr && count % B2_WARPS_PER_CTA == 0;
   if (step)
     if (s->has_convex) b2_step_kernel<3><<<grid, 32 * B2_WARPS_PER_CTA, s->smem_bytes, st>>>(s->hm, s->hd);
     else b2_step_kernel<1><<<grid, 32 * B2_WARPS_PER_CTA, s->smem_bytes, st>>>(s->hm, s->hd);
@@ -470,13 +453,7 @@ static int read_model(const B2ModelDesc* desc, int ncon_per_world, int njmax, co
   if (m.nv > 64 || m.nbody > 64) return fail("b2_create: nv and nbody must be <= 64");
   if (m.nv < 1) return fail("b2_create: model has no degrees of freedom");
   m.integrator = geti("opt_integrator"); m.iterations = geti("opt_iterations");
-  m.ls_iterations = geti("opt_ls_iterations"); m.debug = 8 | 16 | 32;  // bit 3: relative-step stop of the line search; bit 4: shifted warm start after a control
-                         // change; bit 5: the line search evaluates its slope at 0 (off: grad . search and a first trial
-                         // step of 1 - one evaluation fewer per Newton iteration, no measurable time on the GPU, and
-                         // the worst of 1024 stiff envs of the config-C parity states moved from 1.8e-4 to 3.3e-4)
-  m.newton_small = 1e-10f;
-  m.ls_rtol = 1e-3f;  // line search stops once the slope is 1e-3 of its value at 0 (emulated bench workload: 7.0 -> 3.4
-                      // evaluations per Newton iteration, iteration count unchanged: 4.665 -> 4.67)
+  m.ls_iterations = geti("opt_ls_iterations");
   m.timestep = (float)h.scalar("opt_timestep"); m.tolerance = (float)h.scalar("opt_tolerance");
   m.ls_tolerance = (float)h.scalar("opt_ls_tolerance"); m.impratio = (float)h.scalar("opt_impratio");
   m.meaninertia = (float)h.scalar("stat_meaninertia");
@@ -865,23 +842,19 @@ static int shared_memory_layout(b2_sim* s, const HostModel& h) {
   return 0;
 }
 
-// Heavy-first order and work-queue tickets, the step kernel's co-resident CTAs, and the streams of b2_step_n.
+// Heavy-first order, the step kernel's co-resident CTAs, and the streams of b2_step_n.
 static int launch_resources(b2_sim* s) {
   void* p = nullptr;
   if (cudaMalloc(&p, sizeof(int) * (size_t)s->nworld) != cudaSuccess) return fail("cudaMalloc(order)");
   s->allocs.push_back(p);
   s->order = (int*)p;
-  if (cudaMalloc(&p, sizeof(int) * 4) != cudaSuccess) return fail("cudaMalloc(tickets)");
-  s->allocs.push_back(p);
-  s->tickets = (int*)p;
-  cudaMemset(p, 0, sizeof(int) * 4);
   int per_sm = 0, sms = 0;
   // (of the instantiation that steps this model: the convex one has a larger register budget)
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, s->has_convex ? b2_step_kernel<3> : b2_step_kernel<1>,
                                                 32 * B2_WARPS_PER_CTA, s->smem_bytes);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, s->device);
   s->resident_ctas = per_sm * sms;
-  for (int h = 0; h < 4; h++)
+  for (int h = 0; h < 2; h++)
     if (cudaStreamCreateWithFlags(&s->side[h], cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&s->ev_join[h], cudaEventDisableTiming) != cudaSuccess)
       return fail("b2_create: stream/event creation failed");
@@ -940,7 +913,7 @@ int b2_destroy(b2_sim* s) {
   if (!s) return 0;
   DeviceGuard guard(s->device);
   for (void* p : s->allocs) cudaFree(p);
-  for (int h = 0; h < 4; h++) {
+  for (int h = 0; h < 2; h++) {
     if (s->side[h]) cudaStreamDestroy(s->side[h]);
     if (s->ev_join[h]) cudaEventDestroy(s->ev_join[h]);
   }
@@ -1007,7 +980,7 @@ int b2_expand_model_field(b2_sim* s, const char* name, void* stream, B2Tensor* o
 struct OptionRef { int* i; float* f = nullptr; int bit = 0; double scale = 1.0; };  // *f, bit `bit` of *i, or scale * *i
 struct Option {
   const char* name;
-  OptionRef (*ref)(b2_sim*);       // nullptr: accepted and ignored
+  OptionRef (*ref)(b2_sim*);
   bool read_only = false;
   const char* (*refuse)(double) = nullptr;  // optional: why a value is not taken (nullptr when it is)
 };
@@ -1023,17 +996,7 @@ static const Option kOptions[] = {
     {"debug_outputs", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 1}; }},
     {"dense_factor", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 2}; }},  // force the dense LDL schedule (tests)
     {"full_solver", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 4}; }},  // Newton on all dofs even when a leading block suffices (tests, A/B)
-    {"ls_relstep", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 8}; }},  // line search stops on a relative step of a few ulp
-    {"warmstart_shift", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 16}; }},  // previous solution moved by the change of qacc_smooth
-    {"ls_eval0", [](b2_sim* s) { return OptionRef{&s->hm.debug, nullptr, 32}; }},  // evaluate the line-search slope at 0 instead of using grad . search (A/B)
-    {"ls_rtol", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.ls_rtol}; }},
-    {"newton_small", [](b2_sim* s) { return OptionRef{nullptr, &s->hm.newton_small}; }},
-    {"ls_parallel", nullptr},  // accepted for API parity; the line search here is exact
     {"sorted_dispatch", [](b2_sim* s) { return OptionRef{&s->sorted_dispatch}; }},
-    {"fused_decimation", [](b2_sim* s) { return OptionRef{&s->fused_decimation}; }},
-    {"split_streams", [](b2_sim* s) { return OptionRef{&s->split_streams}; }},
-    {"work_queue", [](b2_sim* s) { return OptionRef{&s->work_queue}; }}, {"phase_sync", [](b2_sim* s) { return OptionRef{&s->phase_sync}; }},
-    {"reorder_every_substep", [](b2_sim* s) { return OptionRef{&s->reorder_every_substep}; }},
     {"smem_bytes_per_env", [](b2_sim* s) { return OptionRef{&s->hm.lay.total, nullptr, 0, 4.0}; }, true},
     {"maxcon", [](b2_sim* s) { return OptionRef{&s->hm.maxcon}; }, true},
     {"resident_ctas", [](b2_sim* s) { return OptionRef{&s->resident_ctas}; }, true},
@@ -1050,7 +1013,6 @@ int b2_set_option(b2_sim* s, const char* key, double v) {
   const Option* o = find_option(key);
   if (!o || o->read_only) return fail(std::string("b2_set_option: unknown option '") + key + "'");
   if (o->refuse && o->refuse(v)) return fail(o->refuse(v));
-  if (!o->ref) return 0;
   OptionRef r = o->ref(s);
   if (r.f) *r.f = (float)v;
   else if (r.bit) *r.i = (*r.i & ~r.bit) | ((int)v ? r.bit : 0);
@@ -1060,7 +1022,7 @@ int b2_set_option(b2_sim* s, const char* key, double v) {
 int b2_get_option(b2_sim* s, const char* key, double* v) {
   if (!s || !key || !v) return fail("b2_get_option: bad arguments");
   const Option* o = find_option(key);
-  if (!o || !o->ref) return fail(std::string("b2_get_option: unknown option '") + key + "'");
+  if (!o) return fail(std::string("b2_get_option: unknown option '") + key + "'");
   OptionRef r = o->ref(s);
   *v = r.f ? (double)*r.f : r.bit ? (double)((*r.i & r.bit) != 0) : r.scale * *r.i;
   return 0;
@@ -1091,28 +1053,25 @@ int b2_step_n(b2_sim* s, int n, void* stream) {
   if (n <= 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (refresh_kinrec(s, st)) return 1;
-  if (s->fused_decimation) return launch(s, true, st, n);
-  int np = std::min(std::max(s->split_streams, 1), 4);
-  if (np > 1 && n > 1 && s->nworld >= 1024 * np) {
-    // Environments are independent, so the sub-steps of one partition need not wait for the others:
-    // fork the partitions onto internal streams (event fork/join, CUDA-graph capturable). Each
-    // partition keeps per-sub-step launches (phase-aligned warps, fresh heavy-first order) while
-    // its launch tails overlap the other partitions' work.
-    int per = (((s->nworld + np - 1) / np + B2_WARPS_PER_CTA - 1) / B2_WARPS_PER_CTA) * B2_WARPS_PER_CTA;
+  if (n > 1 && s->nworld >= 2048) {
+    // Environments are independent, so the sub-steps of one half need not wait for the other: fork two
+    // partitions onto internal streams (event fork/join, CUDA-graph capturable). Each partition keeps
+    // per-sub-step launches (phase-aligned warps, fresh heavy-first order) while its launch tails overlap the
+    // other partition's work.  (1, 3 and 4 partitions measured slower on the H100; DESIGN.md §9.)
+    int per = (((s->nworld + 1) / 2 + B2_WARPS_PER_CTA - 1) / B2_WARPS_PER_CTA) * B2_WARPS_PER_CTA;
     CUDA_OK(cudaEventRecord(s->ev_fork, st));
-    for (int h = 0; h < np; h++) {
+    for (int h = 0; h < 2; h++) {
       int base = h * per, count = std::min(per, s->nworld - base);
-      if (count <= 0) break;
       CUDA_OK(cudaStreamWaitEvent(s->side[h], s->ev_fork, 0));
       for (int i = 0; i < n; i++)
-        if (launch(s, true, s->side[h], 1, base, count, h, i == n - 1, i == 0 || s->reorder_every_substep)) return 1;
+        if (launch(s, true, s->side[h], base, count, i == n - 1)) return 1;
       CUDA_OK(cudaEventRecord(s->ev_join[h], s->side[h]));
       CUDA_OK(cudaStreamWaitEvent(st, s->ev_join[h], 0));
     }
     return 0;
   }
   for (int i = 0; i < n; i++)
-    if (launch(s, true, st, 1, 0, -1, 0, i == n - 1, i == 0 || s->reorder_every_substep)) return 1;
+    if (launch(s, true, st, 0, -1, i == n - 1)) return 1;
   return 0;
 }
 
@@ -1182,7 +1141,7 @@ int b2_trackenv_bins(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   return 0;
 }
 
-int b2_step_host(b2_sim* s, const float* ctrl_host, int nsubstep, float* qpos_host, float* qvel_host,
+int b2_step_host(b2_sim* s, const float* ctrl_host, int nsteps, float* qpos_host, float* qvel_host,
                  void* stream) {
   if (!s) return fail("b2_step_host: null sim");
   DeviceGuard guard(s->device);
@@ -1191,7 +1150,7 @@ int b2_step_host(b2_sim* s, const float* ctrl_host, int nsubstep, float* qpos_ho
   if (ctrl_host && m.nu > 0)
     CUDA_OK(cudaMemcpy2DAsync(d.ctrl.p, sizeof(float) * d.ctrl.stride, ctrl_host, sizeof(float) * m.nu,
                               sizeof(float) * m.nu, s->nworld, cudaMemcpyHostToDevice, st));
-  if (nsubstep > 0 && b2_step_n(s, nsubstep, stream)) return 1;
+  if (nsteps > 0 && b2_step_n(s, nsteps, stream)) return 1;
   if (qpos_host)
     CUDA_OK(cudaMemcpy2DAsync(qpos_host, sizeof(float) * m.nq, d.qpos.p, sizeof(float) * d.qpos.stride,
                               sizeof(float) * m.nq, s->nworld, cudaMemcpyDeviceToHost, st));

@@ -84,7 +84,6 @@ class Simulation:
     self._engine = native.Engine(lib, model, num_envs, cfg.nconmax, cfg.njmax, self._dev_index)
     # the env drivers launch their kernels on this library and sim
     self._lib, self._h = lib, self._engine.h
-    self.set_option("ls_parallel", float(cfg.ls_parallel))
 
     opt = SimpleNamespace(
       ls_parallel=cfg.ls_parallel, timestep=float(model.opt_timestep),

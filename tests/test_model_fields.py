@@ -524,11 +524,10 @@ def test_all_fields_randomised_per_world(backend, n, g1_model):
 
 
 @pytest.mark.gpu
-def test_all_fields_randomised_on_every_dispatch_path(g1_model):
+def test_all_fields_randomised_on_partitioned_masked_and_graph_paths(g1_model):
   """2048 G1 worlds, every field per world, against the oracle world by world on each path that remaps or partitions
-  worlds: step_n(4) with default options (two stream partitions of 1024 worlds, each in heavy-first order), the same
-  sub-steps fused into one launch, one step through the work queue, a masked forward, and a CUDA-graph replay after a
-  further model write."""
+  worlds: step_n(4) (two stream partitions of 1024 worlds, each in heavy-first order), a masked forward, and a
+  CUDA-graph replay after a further model write."""
   m = g1_model
   n = 2048
   eng = Eng("cuda", m, n)
@@ -538,7 +537,7 @@ def test_all_fields_randomised_on_every_dispatch_path(g1_model):
   for k in ("iterations",):  # converged answers do not depend on the path that reached them
     eng.set(k, 50)
     o.set_option(k, 50)
-  assert eng.opt("sorted_dispatch") == 1 and eng.opt("split_streams") == 2 and eng.opt("work_queue") == 0
+  assert eng.opt("sorted_dispatch") == 1
   st = make_states(m, n, seed=13)
   load_oracle(o, st)
   for _ in range(4):
@@ -552,22 +551,9 @@ def test_all_fields_randomised_on_every_dispatch_path(g1_model):
     def field(f):
       return ref[f]
 
-  for fused in (0, 1):
-    eng.set("fused_decimation", fused)
-    eng.load(st)
-    eng.step_n(4)
-    check_state(eng, Ref)
-  eng.set("fused_decimation", 0)
-  # one step through the ticket work queue, which is taken when the grid (one CTA per B2_WARPS_PER_CTA = 4 worlds,
-  # csrc/b2_types.h) exceeds the co-resident CTAs
-  assert eng.opt("resident_ctas") < n // 4, eng.opt("resident_ctas")
-  eng.set("work_queue", 1)
-  load_oracle(o, st)
-  o.step()
   eng.load(st)
-  eng.step()
-  check_state(eng, o)
-  eng.set("work_queue", 0)
+  eng.step_n(4)
+  check_state(eng, Ref)
   # masked forward: the unselected worlds keep their outputs bit for bit, the selected ones match the oracle
   st2 = make_states(m, n, seed=14)
   eng.load(st2)

@@ -314,8 +314,8 @@ def test_masked_forward_only_touches_selected_worlds(g1_model):
   sim.close()
 
 
-def test_fused_decimation_matches_separate_steps(g1_model):
-  """b2_step_n(4) (one launch, state kept in shared memory) == 4 x b2_step, bit for bit."""
+def test_step_n_matches_separate_steps(g1_model):
+  """b2_step_n(4) (the last sub-step alone writes the consumer-visible kinematics) == 4 x b2_step, bit for bit."""
   from mjlab_b200.sim import Simulation, SimulationCfg
 
   st = make_states(g1_model, 64, seed=17)
@@ -327,7 +327,6 @@ def test_fused_decimation_matches_separate_steps(g1_model):
   for s in (a, b):
     load_sim(s, st)
     s.data.xfrc_applied[:] = torch.tensor(xf, device="cuda:0")
-  b.set_option("fused_decimation", 1)
   for _ in range(4):
     a.step()
   b.step_n(4)
@@ -335,7 +334,6 @@ def test_fused_decimation_matches_separate_steps(g1_model):
   for f in ("qpos", "qvel", "qacc", "qacc_warmstart", "xpos", "sensordata", "contact_force"):
     assert (getattr(a.data, f)[:] == getattr(b.data, f)[:]).all(), f
   assert torch.allclose(a.data.time[:], b.data.time[:])
-  assert b.launch_count() < a.launch_count()
   a.close()
   b.close()
 
