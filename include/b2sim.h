@@ -116,14 +116,14 @@ int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_ho
 typedef struct B2VelEnvArgs {
   const float* action;            /* [n][nu] */
   const float* U;                 /* [n][B2_VELENV_NU(nu)] uniforms in [0,1): 0-1 reset xy, 2 yaw, 3-5 command, 6 heading
-                                     target, 7 standing draw, 8 command timer, 9-10 push, 11 push timer, 12-15 spare,
-                                     16.. observation noise (9 + 2 nu) */
+                                     target, 7 standing draw, 8 command timer, 9-10 push, 11 push timer, 12 terrain
+                                     level redraw, 13-15 spare, 16.. observation noise (9 + 2 nu) */
   const float* default_qpos;      /* [nq] */
   const float* default_joint_pos; /* [nu] */
   const float* action_scale;      /* [nu] */
   const float* soft_lo;           /* [nu] */
   const float* soft_hi;           /* [nu] */
-  const float* env_origins;       /* [n][3] */
+  float* env_origins;             /* [n][3] spawn origins; in/out with the terrain curriculum, else only read */
   int32_t* episode_length;        /* [n] in/out */
   float* last_action;             /* [n][nu] in/out */
   float* command;                 /* [n][3] in/out */
@@ -140,6 +140,17 @@ typedef struct B2VelEnvArgs {
   float* log_row;                 /* [n][3] out: (reward, terminated, truncated) packed for the rank-0 log gather */
   float step_dt, fall_angle, push_vel, push_lo, push_hi;
   int32_t max_episode_length;
+  /* terrain-level curriculum (terrain_levels_vel, tasks/velocity/mdp/curriculums.py:18-52, and
+   * TerrainImporter.update_env_origins, terrains/terrain_importer.py:186-201); curriculum = 0 leaves every field
+   * below unread. On reset, before the new pose is written: d = |root_xy - origin_xy|, up = d > move_up_dist,
+   * down = d < |command_xy| episode_length_s / 2 and not up; level += up - down; a level >= rows is redrawn as
+   * min(floor(U[12] rows), rows - 1), any other is clipped at 0; env_origins = terrain_origins[level][type]. */
+  const float* terrain_origins;   /* [rows][cols][3] sub-terrain spawn points */
+  int32_t* terrain_levels;        /* [n] in/out: row of each env */
+  const int32_t* terrain_types;   /* [n] column of each env */
+  float* terrain_level_mean;      /* [1] out: mean of terrain_levels after the update (the curriculum's log value) */
+  float move_up_dist, episode_length_s;
+  int32_t rows, cols, curriculum;
 } B2VelEnvArgs;
 int b2_velenv_pre(b2_sim* sim, const float* action, const float* default_joint_pos,
                   const float* action_scale, void* cuda_stream);

@@ -2,8 +2,9 @@
 // 1-3): the caller-side work of ManagerBasedRlEnv.step (reference src/mjlab/envs/manager_based_rl_env.py:106-147
 // with the terms of tasks/velocity/velocity_env_cfg.py) as two kernels instead of ~90 tiny torch launches:
 //   pre  : ctrl = default_joint_pos + action_scale * action                     (joint_actions.py:85-103)
-//   post : episode counter, terminations (bad_orientation, time_out), rewards, masked reset
-//          (events.py:43-124), interval push (events.py:127-143), command resample, observations.
+//   post : episode counter, terminations (bad_orientation, time_out), rewards, the terrain-level curriculum of
+//          the reset envs (opt-in, curriculums.py:18-52), masked reset (events.py:43-124), interval push
+//          (events.py:127-143), command resample, observations.
 // The torch implementation in mjlab_b200/envs/velocity_env.py is the reference; both consume the same
 // per-step uniform numbers U[n][10] so they can be compared exactly (tests/test_boundary_gpu.py).
 #pragma once
@@ -35,6 +36,34 @@ __device__ __forceinline__ float b2e_wsum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// IEEE-rounded products, sums and square roots: the library builds with --use_fast_math (approximate sqrt, FMA
+// contraction), but a terrain level must move exactly as on the torch path
+#ifdef B2_HOST_EMULATION
+__device__ __forceinline__ float b2e_mul_rn(float a, float b) { return a * b; }
+__device__ __forceinline__ float b2e_norm2_rn(float x, float y) { return sqrtf(x * x + y * y); }
+#else
+__device__ __forceinline__ float b2e_mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float b2e_norm2_rn(float x, float y) {
+  return __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
+}
+#endif
+
+// Terrain-level curriculum of a reset env (B2VelEnvArgs, terrain_levels_vel + update_env_origins), on one lane: from
+// the root position (x, y) and the command (c0, c1) of the episode that just ended, move the env's level and write
+// the origin the reset spawns at.
+__device__ __forceinline__ void b2e_terrain_level(const B2VelEnvArgs& A, int w, float x, float y, float c0, float c1,
+                                                  float u) {
+  float* org = A.env_origins + 3 * (size_t)w;
+  const float dist = b2e_norm2_rn(x - org[0], y - org[1]);
+  const bool up = dist > A.move_up_dist;
+  const bool down = !up && dist < b2e_mul_rn(b2e_norm2_rn(c0, c1), A.episode_length_s) * 0.5f;
+  int level = A.terrain_levels[w] + (up ? 1 : 0) - (down ? 1 : 0);
+  level = level >= A.rows ? min((int)floorf(b2e_mul_rn(u, (float)A.rows)), A.rows - 1) : max(level, 0);
+  A.terrain_levels[w] = level;
+  const float* src = A.terrain_origins + 3 * ((size_t)level * A.cols + A.terrain_types[w]);
+  org[0] = src[0]; org[1] = src[1]; org[2] = src[2];
 }
 
 // One warp per environment (a thread per environment left 4096 threads = 128 warps on 132 SMs walking ~400
@@ -89,6 +118,10 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   }
   // masked reset (reset_root_state_uniform + reset_joints_by_scale), command resample
   if (done) {
+    if (A.curriculum) {  // before the reset events (manager_based_rl_env.py:205-208), from the pre-reset state
+      if (lane == 0) b2e_terrain_level(A, w, qpos[0], qpos[1], c0, c1, U[12]);
+      __syncwarp();  // every lane spawns at the new origin
+    }
     for (int i = lane; i < nq; i += 32) {
       float v = A.default_qpos[i];
       if (i == 0) v += (U[0] - 0.5f) + A.env_origins[3 * (size_t)w];
@@ -165,5 +198,29 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     o[9 + a] = jp + (Z[9 + a] * 2.f - 1.f) * 0.01f;
     o[9 + nu + a] = jv + (Z[9 + nu + a] * 2.f - 1.f) * 1.5f;
     o[9 + 2 * nu + a] = la;
+  }
+}
+
+// Mean terrain level after the post kernel's curriculum update, the value terrain_levels_vel returns for logging: one
+// CTA, launched only when the curriculum is on.  The sum of integer levels is exact in any order, so no accumulator
+// has to be zeroed before the post kernel and the value is the same from run to run.
+constexpr int kLevelMeanThreads = 256;
+__global__ void __launch_bounds__(kLevelMeanThreads) b2_velenv_level_mean_kernel(int n, const int32_t* __restrict__ levels,
+                                                                                float* __restrict__ mean) {
+  __shared__ int part[kLevelMeanThreads / 32];
+  int s = 0;
+  for (int i = threadIdx.x; i < n; i += kLevelMeanThreads) s += levels[i];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = 0;
+    for (int k = 0; k < kLevelMeanThreads / 32; k++) s += part[k];
+#ifdef B2_HOST_EMULATION
+    *mean = (float)s / (float)n;
+#else
+    *mean = __fdiv_rn((float)s, (float)n);
+#endif
   }
 }

@@ -1091,11 +1091,22 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
   if (!s || !args) return fail("b2_velenv_post: bad arguments");
   if (s->hm.nq != s->hm.nu + 7 || s->hm.nv != s->hm.nu + 6)
     return fail("b2_velenv_post: expects one floating base plus nu actuated hinge joints");
+  if (args->curriculum &&
+      (!args->env_origins || !args->terrain_origins || !args->terrain_levels || !args->terrain_types ||
+       !args->terrain_level_mean || args->rows < 1 || args->cols < 1))
+    return fail("b2_velenv_post: the terrain curriculum needs env_origins, terrain_origins, terrain_levels, "
+                "terrain_types, terrain_level_mean and rows, cols >= 1");
   DeviceGuard guard(s->device);
   b2_velenv_post_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(  // one warp per environment
       s->hd, s->hm.nq, s->hm.nv, s->hm.nu, *args);
   s->launches++;
   CUDA_OK(cudaGetLastError());
+  if (args->curriculum) {
+    b2_velenv_level_mean_kernel<<<1, kLevelMeanThreads, 0, (cudaStream_t)stream>>>(
+        s->nworld, args->terrain_levels, args->terrain_level_mean);
+    s->launches++;
+    CUDA_OK(cudaGetLastError());
+  }
   return 0;
 }
 

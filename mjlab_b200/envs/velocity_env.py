@@ -15,6 +15,7 @@ import math
 import re
 from dataclasses import dataclass, field
 
+import numpy as np
 import torch
 
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
@@ -34,6 +35,10 @@ class VelocityEnvCfg:
   env_spacing: float = 2.5
   terrain: str = "flat"                    # "flat" (plane) | "rough" (box terrain, velocity_env_cfg.py:274-278)
   max_init_terrain_level: int = 5          # terrain_importer.py:203-223
+  # terrain-level curriculum (velocity_env_cfg.py:228-230, mdp/curriculums.py:18-52): after every episode a robot
+  # moves a row up or down the terrain grid by how far it walked; needs a terrain with sub-terrain origins
+  terrain_curriculum: bool = False
+  terrain_size: tuple = (8.0, 8.0)         # sub-terrain size the model's terrain grid was generated with
   seed: int = 42
   sim: SimulationCfg = field(
     default_factory=lambda: SimulationCfg(
@@ -68,6 +73,9 @@ class VelocityFlatEnv:
     zoo = g1 if cfg.robot == "g1" else go1
     self.model = model if model is not None else load_compiled(f"{cfg.robot}_{cfg.terrain}")
     m = self.model
+    self.terrain_curriculum = bool(cfg.terrain_curriculum)
+    if self.terrain_curriculum and "terrain_origins" not in m.arrays:
+      raise ValueError(f"terrain_curriculum needs a terrain with sub-terrain origins; '{cfg.terrain}' has none")
     self.num_envs = cfg.num_envs
     self.sim = Simulation(cfg.num_envs, cfg.sim, m, device)
     self.nq, self.nv, self.nu = int(m.nq), int(m.nv), int(m.nu)
@@ -93,13 +101,23 @@ class VelocityFlatEnv:
       [(idx // cols - (cols - 1) / 2) * cfg.env_spacing, (idx % cols - (cols - 1) / 2) * cfg.env_spacing,
        torch.zeros(n, device=dev)], dim=1).float()
     if "terrain_origins" in m.arrays:
-      # box terrain: spawn on the sub-terrain origins, level <= max_init_terrain_level, types round-robin
-      # (terrain_importer.py:203-223); the curriculum's level updates are host-side MDP and not restated
+      # sub-terrain grid: spawn on the sub-terrain origins, level <= max_init_terrain_level, types round-robin
+      # (terrain_importer.py:203-223)
       from mjlab_b200.terrains import env_origins_curriculum
 
-      org, self.terrain_levels, self.terrain_types = env_origins_curriculum(
-        n, m.arrays["terrain_origins"], cfg.max_init_terrain_level, cfg.seed)
+      origins = np.asarray(m.arrays["terrain_origins"])
+      # origins sit at the sub-terrain centres, so consecutive rows are one sub-terrain length apart
+      if self.terrain_curriculum and not np.allclose(np.diff(origins[:, :, 0], axis=0), cfg.terrain_size[0]):
+        raise ValueError(f"terrain_size {cfg.terrain_size} does not match the model's terrain grid")
+      org, levels, types = env_origins_curriculum(n, origins, cfg.max_init_terrain_level, cfg.seed)
       self.env_origins = torch.tensor(org, dtype=torch.float32, device=dev)
+      self.terrain_origins = torch.tensor(origins, dtype=torch.float32, device=dev).contiguous()  # [rows, cols, 3]
+      self.terrain_levels = torch.tensor(levels, dtype=torch.int32, device=dev)
+      self.terrain_types = torch.tensor(types, dtype=torch.int32, device=dev)
+      self.max_terrain_level = int(origins.shape[0])
+      self.move_up_dist = 0.5 * float(cfg.terrain_size[0])
+      # the mean level terrain_levels_vel returns for logging, kept on the device (updated by the curriculum)
+      self.terrain_level_mean = self.terrain_levels.float().mean()
     # startup domain randomisation: foot friction (events.py:212-265 'abs' on geom_friction[:, feet, 0])
     self.sim.expand_model_fields(["geom_friction"])
     foot_ids = torch.tensor(
@@ -125,7 +143,7 @@ class VelocityFlatEnv:
     self.push_time_left.copy_(self._rand(n) * (hi_t - lo_t) + lo_t)
     if self.native_mdp:
       self._init_native()
-    self.reset()
+    self._reset_all(curriculum=False)  # no episode has ended yet: the initial levels stand
 
   # -- helpers -----------------------------------------------------------------------------------
   def _rand(self, *shape):
@@ -133,7 +151,8 @@ class VelocityFlatEnv:
 
   def _draw(self) -> torch.Tensor:
     """The step's uniform numbers, one launch (layout: include/b2sim.h B2VelEnvArgs.U): 0-1 reset xy, 2 yaw,
-    3-5 command, 6 heading target, 7 standing draw, 8 command timer, 9-10 push, 11 push timer, 16.. obs noise."""
+    3-5 command, 6 heading target, 7 standing draw, 8 command timer, 9-10 push, 11 push timer, 12 terrain level
+    redraw, 16.. obs noise."""
     return self._rand(self.num_envs, 16 + 9 + 2 * self.nu)
 
   def _init_native(self) -> None:
@@ -165,6 +184,14 @@ class VelocityFlatEnv:
     a.step_dt, a.fall_angle, a.push_vel = self.step_dt, self.cfg.fall_angle, self.cfg.push_vel
     a.push_lo, a.push_hi = self.cfg.push_interval_s
     a.max_episode_length = self.max_episode_length
+    if self.terrain_curriculum:
+      for name, t in (("terrain_origins", self.terrain_origins), ("terrain_levels", self.terrain_levels),
+                      ("terrain_types", self.terrain_types), ("terrain_level_mean", self.terrain_level_mean)):
+        assert t.is_contiguous()
+        setattr(a, name, t.data_ptr())
+      a.move_up_dist, a.episode_length_s = self.move_up_dist, self.cfg.episode_length_s
+      a.rows, a.cols = self.terrain_origins.shape[:2]
+      a.curriculum = 1
     self._native_args = a
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
@@ -185,6 +212,25 @@ class VelocityFlatEnv:
     d.ctrl[:] = torch.where(mk, self.default_joint_pos.expand(n, -1), d.ctrl[:])
     self.episode_length_buf.copy_(torch.where(mask, torch.zeros_like(self.episode_length_buf), self.episode_length_buf))
     self.last_action.copy_(torch.where(mk, torch.zeros_like(self.last_action), self.last_action))
+
+  def _terrain_curriculum(self, mask: torch.Tensor, U: torch.Tensor) -> None:
+    """terrain_levels_vel (tasks/velocity/mdp/curriculums.py:18-52) and TerrainImporter.update_env_origins
+    (terrains/terrain_importer.py:186-201) for the masked envs, from the state of the episode that just ended: a robot
+    that walked further than half a sub-terrain moves a row up, one that walked less than half of what its command
+    asked for moves a row down, one past the last row is redrawn from U[:, 12].  Its reset spawns at the new origin."""
+    o, c, root = self.env_origins, self.command, self.sim.data.qpos[:, 0:2]
+    dx, dy = root[:, 0] - o[:, 0], root[:, 1] - o[:, 1]
+    dist = torch.sqrt(dx * dx + dy * dy)
+    up = dist > self.move_up_dist
+    down = (dist < torch.sqrt(c[:, 0] * c[:, 0] + c[:, 1] * c[:, 1]) * self.cfg.episode_length_s * 0.5) & ~up
+    top = self.max_terrain_level
+    level = self.terrain_levels + up.int() - down.int()
+    redraw = torch.floor(U[:, 12] * top).int().clamp(max=top - 1)
+    level = torch.where(level >= top, redraw, level.clamp(min=0))
+    self.terrain_levels.copy_(torch.where(mask, level, self.terrain_levels))
+    new = self.terrain_origins[self.terrain_levels.long(), self.terrain_types.long()]
+    self.env_origins.copy_(torch.where(mask.unsqueeze(1), new, o))
+    self.terrain_level_mean.copy_(self.terrain_levels.float().mean())
 
   def _update_command(self, done: torch.Tensor, U: torch.Tensor) -> None:
     """CommandTerm.compute + UniformVelocityCommand (tasks/velocity/mdp/velocity_command.py:64-110): resample on
@@ -220,8 +266,15 @@ class VelocityFlatEnv:
 
   # -- API ---------------------------------------------------------------------------------------
   def reset(self):
+    """End every episode and start new ones (with the terrain curriculum on, each env first moves rows by how its
+    episode went)."""
+    return self._reset_all(curriculum=self.terrain_curriculum)
+
+  def _reset_all(self, curriculum: bool):
     all_ = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
     U = self._draw()
+    if curriculum:
+      self._terrain_curriculum(all_, U)
     self._reset_where(all_, U)
     self.sim.forward()
     self._update_command(all_, U)
@@ -296,7 +349,10 @@ class VelocityFlatEnv:
     reward = (r_lin + r_ang + r_pose + r_lim + r_rate) * self.step_dt
     self.last_action.copy_(action)
     done = terminated | truncated
-    # partial reset + forward (manager_based_rl_env.py:128-132), mask-based: no host sync
+    # partial reset + forward (manager_based_rl_env.py:128-132), mask-based: no host sync; the curriculum runs
+    # before the reset events (_reset_idx, :205-208)
+    if self.terrain_curriculum:
+      self._terrain_curriculum(done, U)
     self._reset_where(done, U)
     self._done_buf.copy_(done)
     self.sim.forward(env_mask=self._done_buf)  # only the reset envs need new derived quantities here

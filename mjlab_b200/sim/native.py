@@ -52,6 +52,9 @@ class B2VelEnvArgs(ctypes.Structure):
       "terminated", "truncated", "done", "cmd_time_left", "heading_target", "is_standing", "critic", "log_row")]
     + [(n, ctypes.c_float) for n in ("step_dt", "fall_angle", "push_vel", "push_lo", "push_hi")]
     + [("max_episode_length", ctypes.c_int32)]
+    + [(n, ctypes.c_void_p) for n in ("terrain_origins", "terrain_levels", "terrain_types", "terrain_level_mean")]
+    + [(n, ctypes.c_float) for n in ("move_up_dist", "episode_length_s")]
+    + [(n, ctypes.c_int32) for n in ("rows", "cols", "curriculum")]
   )
 
 
