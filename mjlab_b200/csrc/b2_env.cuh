@@ -6,7 +6,8 @@
 //          the reset envs (opt-in, curriculums.py:18-52), masked reset (events.py:43-124), interval push
 //          (events.py:127-143), command resample, observations.
 // The torch implementation in mjlab_b200/envs/velocity_env.py is the reference; both consume the same
-// per-step uniform numbers U[n][10] so they can be compared exactly (tests/test_boundary_gpu.py).
+// per-step uniform numbers U[n][B2_VELENV_NU(nu)] (layout in include/b2sim.h) so they can be compared on one state
+// (tests/test_mdp_kernels.py).
 #pragma once
 #include "../../include/b2sim.h"
 #include "b2_types.h"

@@ -406,13 +406,27 @@ class TrackingFlatEnv:
     if getattr(self, "_native_args", None) is None:
       self._native_setup()
     sim = self.sim
-    st = sim._stream()
     self._U.copy_(U)
     self._act.copy_(action)
     native.check(sim._lib.b2_velenv_pre(sim._h, ctypes.c_void_p(self._act.data_ptr()),
                                         ctypes.c_void_p(self.default_joint_pos.data_ptr()),
-                                        ctypes.c_void_p(self.action_scale.data_ptr()), st))
+                                        ctypes.c_void_p(self.action_scale.data_ptr()), sim._stream()))
     sim.step_n(self.cfg.decimation)
+    return self._mdp_native(self._act, self._U)
+
+  def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
+    """Everything after the sub-steps on the fused path: post1 (and the sampler's bins), the forward of the reset
+    envs, post2."""
+    import ctypes
+
+    if getattr(self, "_native_args", None) is None:
+      self._native_setup()
+    sim = self.sim
+    st = sim._stream()
+    if action is not self._act:  # (the kernels read their own two input buffers)
+      self._act.copy_(action)
+    if U is not self._U:
+      self._U.copy_(U)
     native.check(sim._lib.b2_trackenv_post1(sim._h, ctypes.byref(self._native_args), st))
     if self.start_mode == native.START_ADAPTIVE:
       native.check(sim._lib.b2_trackenv_bins(sim._h, ctypes.byref(self._native_args), st))
@@ -421,10 +435,16 @@ class TrackingFlatEnv:
     return self._obs, self._reward, self._term, self._trunc, self._extras(self._critic)
 
   def _step_torch(self, action: torch.Tensor, U: torch.Tensor):
+    self.sim.data.ctrl[:] = self.default_joint_pos + self.action_scale * action  # JointPositionAction, use_default_offset
+    self.sim.step_n(self.cfg.decimation)
+    return self._mdp_torch(action, U)
+
+  def _mdp_torch(self, action: torch.Tensor, U: torch.Tensor):
+    """Everything after the sub-steps, in torch ops on the env's own tensors.  It returns fresh tensors and leaves the
+    fused path's output buffers alone, so an env built with ``native_mdp=True`` can run it too (the tests compare the
+    two on one state)."""
     cfg, d, n, nu = self.cfg, self.sim.data, self.num_envs, self.nu
     S = 13 + nu
-    d.ctrl[:] = self.default_joint_pos + self.action_scale * action  # JointPositionAction, use_default_offset
-    self.sim.step_n(cfg.decimation)
     self.episode_length_buf += 1
     pos, quat, lin, ang = self._robot_bodies()
     a_pos = self._clip("body_pos_w")[:, self.anchor] + self.env_origins

@@ -317,22 +317,40 @@ class VelocityFlatEnv:
     sim = self.sim
     self._action_in.copy_(action)
     self._U.copy_(self._draw())
-    st = sim._stream()
     native.check(sim._lib.b2_velenv_pre(
       sim._h, ctypes.c_void_p(self._action_in.data_ptr()), ctypes.c_void_p(self.default_joint_pos.data_ptr()),
-      ctypes.c_void_p(self.action_scale.data_ptr()), st))
+      ctypes.c_void_p(self.action_scale.data_ptr()), sim._stream()))
     sim.step_n(self.cfg.decimation)
-    native.check(sim._lib.b2_velenv_post(sim._h, ctypes.byref(self._native_args), st))
+    return self._mdp_native(self._action_in, self._U)
+
+  def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
+    """Everything after the sub-steps on the fused path: b2_velenv_post, then the forward of the reset envs."""
+    import ctypes
+
+    from mjlab_b200.sim import native
+
+    sim = self.sim
+    if action is not self._action_in:  # (the kernel reads its own two input buffers)
+      self._action_in.copy_(action)
+    if U is not self._U:
+      self._U.copy_(U)
+    native.check(sim._lib.b2_velenv_post(sim._h, ctypes.byref(self._native_args), sim._stream()))
     sim.forward(env_mask=self._done_buf)
     return self._obs, self._reward, self._term, self._trunc, {"critic": self._critic}
 
   def _step_torch(self, action: torch.Tensor):
     """Reference implementation of the same step in torch ops (also the checker of the fused kernels)."""
-    cfg, d = self.cfg, self.sim.data
     U = self._draw()
     # JointPositionAction: target = default + scale * action (joint_actions.py:85-103)
-    d.ctrl[:] = self.default_joint_pos + self.action_scale * action
-    self.sim.step_n(cfg.decimation)
+    self.sim.data.ctrl[:] = self.default_joint_pos + self.action_scale * action
+    self.sim.step_n(self.cfg.decimation)
+    return self._mdp_torch(action, U)
+
+  def _mdp_torch(self, action: torch.Tensor, U: torch.Tensor):
+    """Everything after the sub-steps, in torch ops on the env's own tensors.  It returns fresh tensors and leaves the
+    fused path's output buffers alone, so an env built with ``native_mdp=True`` can run it too (the tests compare the
+    two on one state)."""
+    cfg, d = self.cfg, self.sim.data
     self.episode_length_buf += 1
     q = d.qpos[:, 3:7]
     grav_b = quat_rotate_inverse(q, self._down)

@@ -271,8 +271,10 @@ def test_entity_data_over_engine_views(g1_model):
 
 
 def test_native_mdp_kernels_match_torch_reference():
-  """b2_velenv_pre/post (fused MDP glue) vs the torch implementation, same seeds and uniforms: terminations,
-  rewards, masked resets, pushes, command resampling and observations agree step by step."""
+  """b2_velenv_pre/post (fused MDP glue) vs the torch implementation through step() end to end, same seeds and
+  uniforms.  Two simulations run the physics separately and b is re-synchronised to a after every step, so this
+  comparison is loose (an agreement fraction, absolute tolerances); the strict one, on one saved state, every output
+  and every environment, is tests/test_mdp_kernels.py."""
   from mjlab_b200.envs import VelocityEnvCfg, VelocityFlatEnv
 
   cfg = dict(num_envs=128, fall_angle=0.12, push_interval_s=(0.02, 0.08), episode_length_s=0.2)

@@ -267,7 +267,9 @@ class EmulSimulation:
 
 def test_emulated_env_native_mdp_kernels_match_torch_reference(monkeypatch):
   """The velocity env on the emulated library: the fused MDP kernels (b2_velenv_pre / b2_velenv_post) against the
-  torch implementation of the same step - terminations, rewards, masked resets, pushes, observations - on CPU."""
+  torch implementation through step() end to end, on CPU.  Two simulations run the physics separately and are
+  re-synchronised after every step, so the tolerances are loose; the strict comparison, on one saved state, is
+  tests/test_mdp_kernels.py."""
   import torch
 
   import mjlab_b200.envs.velocity_env as ve
@@ -301,8 +303,9 @@ def test_emulated_env_native_mdp_kernels_match_torch_reference(monkeypatch):
 
 def test_emulated_tracking_env_native_mdp_kernels_match_torch_reference(monkeypatch):
   """The tracking env (config C) on the emulated library: the fused MDP kernels (csrc/b2_trackenv.cuh) against the
-  torch implementation of the same step - terminations, rewards, RSI resets, clip restarts, anchor-relative targets,
-  pushes, policy and critic observations - on CPU, consuming the same uniforms."""
+  torch implementation through step() end to end, on CPU, consuming the same uniforms.  Two simulations run the
+  physics separately and are re-synchronised after every step, so the tolerances are loose; the strict comparison, on
+  one saved state, is tests/test_mdp_kernels.py."""
   import torch
 
   import mjlab_b200.envs.tracking_env as te

@@ -92,8 +92,10 @@ def test_tracking_env_step_is_graph_capturable():
 
 
 def test_tracking_native_mdp_kernels_match_torch_reference():
-  """csrc/b2_trackenv.cuh (two fused kernels around the masked forward) against the torch implementation of the same
-  env step on the same uniforms: terminations, rewards, RSI resets, clip restarts, targets, pushes, observations."""
+  """csrc/b2_trackenv.cuh (two fused kernels around the masked forward) against the torch implementation through
+  step() end to end, on the same uniforms.  Two simulations run the physics separately and are re-synchronised after
+  every step, so this comparison is loose; the strict one, on one saved state, every output and every environment, is
+  tests/test_mdp_kernels.py."""
   from mjlab_b200.envs import TrackingEnvCfg, TrackingFlatEnv
 
   n = 128
