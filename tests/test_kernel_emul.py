@@ -361,8 +361,9 @@ def _limb(name, n, pos, axes):
 
 
 def test_emulated_kernel_synthetic_45dof_robot(lib):
-  """Sizes no GPU test reaches: a 45-dof, 41-body floating base with five 7-8 joint limbs, 781 collision pairs,
-  self-collisions (dense factorisation schedule), ~40 contacts / ~160 constraint rows per world."""
+  """A 45-dof, 41-body floating base with five 7-8 joint limbs, 781 collision pairs, self-collisions (dense
+  factorisation schedule), ~40 contacts / ~160 constraint rows per world, on the host; the product build is checked at
+  these sizes and beyond (nv and nbody up to 64) by tests/test_model_shapes_gpu.py."""
   from mjlab_b200.compiler import Spec
 
   xml = f"""<mujoco><compiler angle="radian"/><option timestep="0.004" integrator="implicitfast"/>

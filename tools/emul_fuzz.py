@@ -18,54 +18,9 @@ sys.path[:0] = [str(ROOT), str(ROOT / "tests"), str(ROOT / "tests" / "emul")]
 
 from mjlab_b200.compiler import Spec  # noqa: E402
 from oracle.oracle import Oracle  # noqa: E402
+from synth_models import robot_xml  # noqa: E402
 from test_kernel_emul import EmulSim, _load  # noqa: E402
 from util import relerr  # noqa: E402
-
-
-def robot_xml(rng, limbs, joints):
-  """Random articulated robot: hinge / slide joints, limits, per-geom margin, gap, condim, friction, solref /
-  solimp variations, position actuators with force ranges on a third of the joints, Euler or implicitfast."""
-  axes = ["1 0 0", "0 1 0", "0 0 1"]
-  body, acts = "", ""
-  budget = 58
-  for li in range(limbs):
-    n = int(min(budget, rng.integers(max(1, joints - 3), joints + 1)))
-    budget -= n
-    ang = 2 * np.pi * li / limbs
-    pos = f"{0.2 * np.cos(ang):.3f} {0.15 * np.sin(ang):.3f} -0.06"
-    s, close = "", ""
-    for k in range(n):
-      # children are offset sideways: exactly coincident capsule axes give zero-length contact normals,
-      # which no implementation defines
-      p = pos if k == 0 else f"{rng.uniform(-0.03, 0.03):.3f} {rng.uniform(-0.03, 0.03):.3f} -0.12"
-      ax = axes[int(rng.integers(0, 3))]
-      slide = rng.uniform() < 0.15
-      jt = 'type="slide" range="-0.05 0.05"' if slide else 'range="-1.2 1.2"'
-      gopt = ""
-      if rng.uniform() < 0.3:
-        gopt += f' margin="{rng.uniform(0.0, 0.01):.4f}" gap="{rng.uniform(0.0, 0.004):.4f}"'
-      if rng.uniform() < 0.3:
-        gopt += ' condim="1"'
-      if rng.uniform() < 0.3:
-        gopt += f' friction="{rng.uniform(0.2, 1.5):.2f} 0.005 0.0001"'
-      u = rng.uniform()
-      if u < 0.25:
-        gopt += f' solref="{rng.uniform(0.01, 0.05):.3f} {rng.uniform(0.7, 1.3):.2f}" solimp="0.8 0.97 0.002 0.4 {rng.uniform(1, 3):.1f}"'
-      elif u < 0.35:
-        gopt += ' solref="-2000 -50"'
-      s += (f'<body name="l{li}_{k}" pos="{p}"><joint name="j{li}_{k}" axis="{ax}" {jt} limited="true" '
-            f'damping="{rng.uniform(0.0, 0.5):.2f}" armature="0.01"/>'
-            f'<geom type="capsule" fromto="0 0 0 0 0 -0.12" size="0.03" mass="0.4"{gopt}/>')
-      close += "</body>"
-      if rng.uniform() < 0.33:
-        fr = f' forcerange="-{rng.uniform(2, 20):.1f} {rng.uniform(2, 20):.1f}" forcelimited="true"' if rng.uniform() < 0.5 else ""
-        acts += f'<position joint="j{li}_{k}" kp="{rng.uniform(5, 80):.1f}" kv="{rng.uniform(0.1, 3):.2f}"{fr}/>'
-    body += s + close
-  integ = ["implicitfast", "Euler"][int(rng.integers(0, 2))]
-  return f"""<mujoco><compiler angle="radian"/><option timestep="0.004" integrator="{integ}"/>
-  <worldbody><geom name="floor" type="plane" size="0 0 1"/>
-  <body name="base" pos="0 0 0.55"><freejoint/><geom type="box" size="0.2 0.15 0.06" mass="4"/>{body}</body>
-  </worldbody><actuator>{acts}</actuator></mujoco>"""
 
 
 def obstacle_runs(lib, seeds, worlds, steps, keep_going=False):
