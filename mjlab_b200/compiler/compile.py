@@ -589,16 +589,20 @@ def compile_spec(spec: S.Spec) -> Model:
     A["actuator_gear"].append(a.gear)
   nu = len(spec.actuators)
 
-  # ---- sensors (contact sensors only; others keep their slot but read 0) -----------------
+  # ---- sensors (contact sensors only) ----------------------------------------------------
   adr = 0
   kind_of = {S.OBJ_BODY: "body", S.OBJ_XBODY: "body", S.OBJ_GEOM: "geom", S.OBJ_SITE: "site"}
   for k, sn in enumerate(spec.sensors):
-    if sn.type == S.SENS_MJCF:  # (declared in MJCF; contact sensors arrive through add_sensor / ContactSensorCfg)
+    # contact sensors arrive through add_sensor: ContactSensorCfg's default type, or MuJoCo's mjSENS_CONTACT from
+    # the reference's ContactSensorCfg on the MjSpec stand-in; anything else (an MJCF declaration, or add_sensor
+    # with another mjtSensor type) is refused rather than evaluated as a contact sensor
+    if sn.type not in (S.SENS_CONTACT, S.MJ_SENS_CONTACT):
+      what = f"<{sn.tag or 'sensor'}>" if sn.type == S.SENS_MJCF else f"type {sn.type}"
       raise NotImplementedError(
-        f"sensor '{sn.name}' (<{sn.tag or 'sensor'}>): the engine evaluates contact sensors only (SURVEY.md §8a P9)")
+        f"sensor '{sn.name}' ({what}): the engine evaluates contact sensors only (SURVEY.md §8a P9)")
     sn.id = k
     names["sensor"].append(sn.name)
-    A["sensor_type"].append(sn.type)
+    A["sensor_type"].append(S.SENS_CONTACT)  # (one id, whichever way the sensor was added)
     A["sensor_objtype"].append(sn.objtype)
     A["sensor_objid"].append(names[kind_of[sn.objtype]].index(sn.objname))
     A["sensor_reftype"].append(sn.reftype)

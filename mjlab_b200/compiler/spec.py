@@ -46,6 +46,7 @@ GEOM_TYPES = {
 JNT_TYPES = {"free": JNT_FREE, "ball": JNT_BALL, "slide": JNT_SLIDE, "hinge": JNT_HINGE}
 OBJ_BODY, OBJ_XBODY, OBJ_GEOM, OBJ_SITE = 1, 2, 5, 6
 SENS_CONTACT = 100  # private id; only contact sensors are evaluated by the engine
+MJ_SENS_CONTACT = 42  # mjtSensor.mjSENS_CONTACT, as the reference's ContactSensorCfg passes it to add_sensor
 SENS_MJCF = 101     # any sensor declared in MJCF (<sensor><jointpos .../> ...): listed by name, refused by compile()
 OBJ_UNKNOWN = 0
 INT_EULER, INT_IMPLICITFAST = 0, 3

@@ -2553,6 +2553,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
       int rt = m.sensor_reftype[sidx], ri = m.sensor_refid[sidx];
       #pragma unroll 1
       for (int k = lane; k < sdim; k += 32) sd[adr + k] = 0.f;
+      __syncwarp();  // (orders the zeroing before another lane's slot writes to the same addresses)
       int nmatch = 0;
       float net[3] = {0.f, 0.f, 0.f}, wp[3] = {0.f, 0.f, 0.f}, wsm = 0.f;
       #pragma unroll 1

@@ -61,18 +61,18 @@ class Eng:
   """One b2_sim on either backend.  Fields are fetched afresh on every access (an expansion moves a model field), as
   torch tensors over engine memory: device memory on "cuda", host memory on "emul"."""
 
-  def __init__(self, backend, model, n):
+  def __init__(self, backend, model, n, nconmax=None):
     self.n = n
     if backend == "emul":
       from engine import host_tensor
 
-      self.sim, self.e, self.dev = None, native.Engine(_emul_lib(), model, n), "cpu"
+      self.sim, self.e, self.dev = None, native.Engine(_emul_lib(), model, n, nconmax), "cpu"
       self._wrap = host_tensor
     else:
       from mjlab_b200.sim import Simulation, SimulationCfg
       from mjlab_b200.sim.sim_data import tensor_from_b2
 
-      self.sim = Simulation(n, SimulationCfg(), model, "cuda:0")
+      self.sim = Simulation(n, SimulationCfg(nconmax=nconmax), model, "cuda:0")
       self.e, self.dev = self.sim._engine, "cuda:0"
       self._wrap = lambda t: tensor_from_b2(t, self.sim)
     self.lib, self.h = self.e.lib, self.e.h

@@ -69,10 +69,11 @@ def relerr(a, b, floor=1e-9):
   return np.abs(a - b).max(axis=1) / np.maximum(np.abs(b).max(axis=1), floor)
 
 
-def convex_scene():
+def convex_scene(sensors=()):
   """Scene that exercises every mesh / height-field pair type of csrc/b2_convex.h: a ground plane, a wavy height
   field, and free bodies carrying mesh, box, sphere and capsule geoms — one cluster over the plane (plane-mesh,
-  mesh-mesh, box-mesh, sphere-mesh, capsule-mesh) and one over the field (hfield-sphere/capsule/box/mesh)."""
+  mesh-mesh, box-mesh, sphere-mesh, capsule-mesh) and one over the field (hfield-sphere/capsule/box/mesh).
+  `sensors`: ContactSensorCfg-like editors applied to the spec before it is compiled."""
   from mjlab_b200.compiler.spec import Spec
 
   rng = np.random.default_rng(7)
@@ -106,6 +107,8 @@ def convex_scene():
   body("hc", [4.3, 0.4, 0.0], type="capsule", size=[0.05, 0.15])
   body("hb", [4.5, -0.5, 0.0], type="box", size=[0.12, 0.09, 0.06])
   body("hm", [3.5, 0.5, 0.0], type="mesh", meshname="poly1")
+  for s in sensors:
+    s.edit_spec(spec)
   m = spec.compile()
   hf = dict(pos=np.array([4.0, 0.0, 0.0]), size=np.array([1.6, 1.2, 0.25, 0.1]), data=np.clip(elev, 0, 1))
   return m, anchors, hf
