@@ -15,6 +15,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass, field
+from typing import NamedTuple
 
 import numpy as np
 
@@ -23,41 +24,49 @@ from mjlab_b200.compiler.spec import quat_mul, quat_to_mat, mat_to_quat
 
 MINVAL = 1e-15
 
-# (name, dtype) of every array that travels through the C ABI (include/b2sim.h: B2Array).
-# "f" arrays are float64 on the host; the CUDA library narrows them to fp32 on upload.
-MODEL_ARRAYS = [
-  ("body_parentid", "i"), ("body_rootid", "i"), ("body_weldid", "i"),
-  ("body_jntadr", "i"), ("body_jntnum", "i"), ("body_dofadr", "i"), ("body_dofnum", "i"),
-  ("body_pos", "f"), ("body_quat", "f"), ("body_ipos", "f"), ("body_iquat", "f"),
-  ("body_mass", "f"), ("body_subtreemass", "f"), ("body_inertia", "f"),
-  ("body_invweight0", "f"),
-  ("jnt_type", "i"), ("jnt_qposadr", "i"), ("jnt_dofadr", "i"), ("jnt_bodyid", "i"),
-  ("jnt_limited", "i"), ("jnt_pos", "f"), ("jnt_axis", "f"), ("jnt_range", "f"),
-  ("jnt_solref", "f"), ("jnt_solimp", "f"), ("jnt_margin", "f"), ("jnt_stiffness", "f"),
-  ("dof_bodyid", "i"), ("dof_jntid", "i"), ("dof_parentid", "i"),
-  ("dof_armature", "f"), ("dof_damping", "f"), ("dof_frictionloss", "f"),
-  ("dof_invweight0", "f"),
-  ("geom_type", "i"), ("geom_bodyid", "i"), ("geom_contype", "i"),
-  ("geom_conaffinity", "i"), ("geom_condim", "i"), ("geom_priority", "i"),
-  ("geom_size", "f"), ("geom_pos", "f"), ("geom_quat", "f"), ("geom_friction", "f"),
-  ("geom_solref", "f"), ("geom_solimp", "f"), ("geom_solmix", "f"), ("geom_margin", "f"),
-  ("geom_gap", "f"), ("geom_rbound", "f"), ("geom_rgba", "f"),
-  ("site_bodyid", "i"), ("site_pos", "f"), ("site_quat", "f"),
-  ("actuator_trnid", "i"), ("actuator_ctrllimited", "i"), ("actuator_forcelimited", "i"),
-  ("actuator_gainprm", "f"), ("actuator_biasprm", "f"), ("actuator_ctrlrange", "f"),
-  ("actuator_forcerange", "f"), ("actuator_gear", "f"),
-  ("pair_geom1", "i"), ("pair_geom2", "i"),
+
+class ModelArray(NamedTuple):
+  name: str
+  dtype: type  # float64 arrays are narrowed to fp32 by the CUDA library on upload
+  width: int | None = None  # row width of a 2-D array; None: 1-D
+  set_const: bool = False  # computed by _set_const from the packed model, not by a compile stage
+
+
+# Every array that travels through the C ABI (include/b2sim.h: B2Array), in descriptor order.
+I, F, SET_CONST = np.int32, np.float64, True
+MODEL_ARRAYS = [ModelArray(*row) for row in [
+  ("body_parentid", I), ("body_rootid", I), ("body_weldid", I),
+  ("body_jntadr", I), ("body_jntnum", I), ("body_dofadr", I), ("body_dofnum", I),
+  ("body_pos", F, 3), ("body_quat", F, 4), ("body_ipos", F, 3), ("body_iquat", F, 4),
+  ("body_mass", F), ("body_subtreemass", F, None, SET_CONST), ("body_inertia", F, 3),
+  ("body_invweight0", F, 2, SET_CONST),
+  ("jnt_type", I), ("jnt_qposadr", I), ("jnt_dofadr", I), ("jnt_bodyid", I),
+  ("jnt_limited", I), ("jnt_pos", F, 3), ("jnt_axis", F, 3), ("jnt_range", F, 2),
+  ("jnt_solref", F, 2), ("jnt_solimp", F, 5), ("jnt_margin", F), ("jnt_stiffness", F),
+  ("dof_bodyid", I), ("dof_jntid", I), ("dof_parentid", I),
+  ("dof_armature", F), ("dof_damping", F), ("dof_frictionloss", F),
+  ("dof_invweight0", F, None, SET_CONST),
+  ("geom_type", I), ("geom_bodyid", I), ("geom_contype", I),
+  ("geom_conaffinity", I), ("geom_condim", I), ("geom_priority", I),
+  ("geom_size", F, 3), ("geom_pos", F, 3), ("geom_quat", F, 4), ("geom_friction", F, 3),
+  ("geom_solref", F, 2), ("geom_solimp", F, 5), ("geom_solmix", F), ("geom_margin", F),
+  ("geom_gap", F), ("geom_rbound", F), ("geom_rgba", F, 4),
+  ("site_bodyid", I), ("site_pos", F, 3), ("site_quat", F, 4),
+  ("actuator_trnid", I), ("actuator_ctrllimited", I), ("actuator_forcelimited", I),
+  ("actuator_gainprm", F, 10), ("actuator_biasprm", F, 10), ("actuator_ctrlrange", F, 2),
+  ("actuator_forcerange", F, 2), ("actuator_gear", F),
+  ("pair_geom1", I), ("pair_geom2", I),
   # static (world-welded, non-plane) collision geoms found through a uniform xy grid instead of the pair table
-  ("static_geom", "i"), ("static_cell0", "i"), ("dyn_cgeom", "i"), ("grid_start", "i"), ("grid_items", "i"),
-  ("grid_params", "f"),
+  ("static_geom", I), ("static_cell0", I, 2), ("dyn_cgeom", I), ("grid_start", I), ("grid_items", I),
+  ("grid_params", F),
   # mesh / height-field assets (csrc/b2_convex.h): geom_dataid -> mesh id (mesh geoms) or hfield id (hfield geoms)
-  ("geom_dataid", "i"), ("mesh_vertadr", "i"), ("mesh_vertnum", "i"), ("mesh_vert", "f"),
-  ("hfield_adr", "i"), ("hfield_nrow", "i"), ("hfield_ncol", "i"), ("hfield_size", "f"), ("hfield_data", "f"),
-  ("sensor_type", "i"), ("sensor_objtype", "i"), ("sensor_objid", "i"),
-  ("sensor_reftype", "i"), ("sensor_refid", "i"), ("sensor_intprm", "i"),
-  ("sensor_adr", "i"), ("sensor_dim", "i"),
-  ("qpos0", "f"),
-]
+  ("geom_dataid", I), ("mesh_vertadr", I), ("mesh_vertnum", I), ("mesh_vert", F, 3),
+  ("hfield_adr", I), ("hfield_nrow", I), ("hfield_ncol", I), ("hfield_size", F, 4), ("hfield_data", F),
+  ("sensor_type", I), ("sensor_objtype", I), ("sensor_objid", I),
+  ("sensor_reftype", I), ("sensor_refid", I), ("sensor_intprm", I, 3),
+  ("sensor_adr", I), ("sensor_dim", I),
+  ("qpos0", F),
+]]
 MODEL_SCALARS_I = [
   "nq", "nv", "nu", "nbody", "njnt", "ngeom", "nsite", "nsensor", "nsensordata", "npair", "nstatic",
   "opt_integrator", "opt_cone", "opt_solver", "opt_iterations", "opt_ls_iterations",
@@ -65,6 +74,8 @@ MODEL_SCALARS_I = [
 MODEL_SCALARS_F = [
   "opt_timestep", "opt_tolerance", "opt_ls_tolerance", "opt_impratio", "stat_meaninertia",
 ]
+# (qpos width, dof width) of each joint type the engine compiles (ball joints are refused)
+JOINT_WIDTH = {S.JNT_FREE: (7, 6), S.JNT_SLIDE: (1, 1), S.JNT_HINGE: (1, 1)}
 
 
 class _Accessor:
@@ -99,7 +110,7 @@ class Model:
   def body(self, name):
     i = int(name) if isinstance(name, (int, np.integer)) else self.name2id("body", name)
     return _Accessor(id=i, name=self.names["body"][i], mass=np.array([float(self.body_mass[i])]),
-                     pos=np.asarray(self.body_pos).reshape(-1, 3)[i], parentid=np.array([int(self.body_parentid[i])]))
+                     pos=np.asarray(self.body_pos)[i], parentid=np.array([int(self.body_parentid[i])]))
 
   # (scalar attributes come back as 1-element arrays, as the MuJoCo bindings return them: `jnt.dofadr[0]`)
   def joint(self, name):
@@ -107,7 +118,7 @@ class Model:
     return _Accessor(
       id=i, name=self.names["joint"][i], type=np.array([int(self.jnt_type[i])]),
       qposadr=np.array([int(self.jnt_qposadr[i])]), dofadr=np.array([int(self.jnt_dofadr[i])]),
-      range=np.asarray(self.jnt_range).reshape(-1, 2)[i],
+      range=np.asarray(self.jnt_range)[i],
     )
 
   def geom(self, key):
@@ -157,7 +168,6 @@ class Model:
     meta = json.loads(str(z["__meta__"]))
     m = Model()
     m.arrays = {k: z[k] for k in z.files if k != "__meta__"}
-    fill_asset_defaults(m.arrays)
     m.names = meta["names"]
     m.keys = {
       k: {n: (None if v is None else np.array(v)) for n, v in d.items()}
@@ -165,18 +175,6 @@ class Model:
     }
     m.opt_gravity = np.array(meta["gravity"])
     return m
-
-
-def fill_asset_defaults(arrays: dict) -> None:
-  """Model tables written before mesh / height-field assets existed (compiled blobs, MjModel-like objects
-  without assets) get empty asset arrays and ``geom_dataid = -1``."""
-  if "geom_dataid" not in arrays:
-    arrays["geom_dataid"] = np.full(int(np.asarray(arrays["ngeom"]).reshape(-1)[0]), -1, dtype=np.int32)
-  for k, dt in (("mesh_vertadr", np.int32), ("mesh_vertnum", np.int32), ("mesh_vert", np.float64),
-                ("hfield_adr", np.int32), ("hfield_nrow", np.int32), ("hfield_ncol", np.int32),
-                ("hfield_size", np.float64), ("hfield_data", np.float64)):
-    if k not in arrays:
-      arrays[k] = np.zeros((0, 3) if k == "mesh_vert" else ((0, 4) if k == "hfield_size" else 0), dtype=dt)
 
 
 # ---------------------------------------------------------------------------------------
@@ -398,169 +396,174 @@ def _build_static_grid(A, static, weld, gbody, gtype, ngeom, cell: float = 1.0) 
 
 
 def compile_spec(spec: S.Spec) -> Model:
-  bodies = spec.bodies
-  for i, b in enumerate(bodies):
-    b.id = i
-  nbody = len(bodies)
-  A: dict[str, list] = {k: [] for k, _ in MODEL_ARRAYS}
+  """The compile stages in order: they fill ``A`` (a list per MODEL_ARRAYS row) and ``names``; ``_pack`` makes the Model."""
+  A: dict[str, list] = {a.name: [] for a in MODEL_ARRAYS}
   names = {k: [] for k in ("body", "joint", "geom", "site", "actuator", "sensor")}
+  mesh_ids, hfield_ids = {}, {}  # asset name -> mesh / height-field id
+  # one depth-first pass: the ids of each element kind, and the first refusal among them, follow body order
+  for b in spec.bodies:
+    _body(spec, b, A, names)
+    _joints(spec, b, A, names)
+    _geoms(spec, b, A, names, mesh_ids, hfield_ids)
+    _sites(b, A, names)
+  _weld_and_root(A)
+  _actuators(spec, A, names)
+  _contact_sensors(spec, A, names)
+  _collision_pairs(spec, A, names)
+  _refuse_unsupported(A, names)
+  m = _pack(spec, A, names)
+  _set_const(m)
+  _keyframes(spec, m)
+  return m
 
-  # ---- bodies, joints, dofs ------------------------------------------------------------
-  nq = nv = 0
-  jid = gid = sid = 0
-  dof_last_of_body = {}
-  qpos0 = []
-  mesh_ids: dict[str, int] = {}
-  hfield_ids: dict[str, int] = {}
-  for b in bodies:
-    names["body"].append(b.name)
-    pid = b.parent.id if b.parent is not None else 0
-    A["body_parentid"].append(pid)
-    A["body_pos"].append(b.pos)
-    A["body_quat"].append(b.quat / np.linalg.norm(b.quat))
-    if b.mass is not None:
-      ipos, iquat, mass, inertia = b.ipos, b.iquat, b.mass, b.inertia
-    else:
-      ipos, iquat, mass, inertia = _body_inertial_from_geoms(b, spec.meshes)
-    A["body_ipos"].append(ipos)
-    A["body_iquat"].append(iquat / np.linalg.norm(iquat))
-    A["body_mass"].append(mass)
-    A["body_inertia"].append(inertia)
-    A["body_jntadr"].append(jid if b.joints else -1)
-    A["body_jntnum"].append(len(b.joints))
-    A["body_dofadr"].append(nv if b.joints else -1)
-    ndof_b = 0
-    # dof chain parent: last dof of the nearest ancestor that has dofs
-    anc = b.parent
-    par_dof = -1
-    while anc is not None:
-      if anc.id in dof_last_of_body:
-        par_dof = dof_last_of_body[anc.id]
-        break
-      anc = anc.parent
-    for j in b.joints:
-      j.id = jid
-      names["joint"].append(j.name)
-      A["jnt_type"].append(j.type)
-      A["jnt_qposadr"].append(nq)
-      A["jnt_dofadr"].append(nv)
-      A["jnt_bodyid"].append(b.id)
-      A["jnt_pos"].append(j.pos)
-      A["jnt_axis"].append(j.axis)
-      limited = j.limited
-      if limited == 2:
-        limited = int(spec.autolimits and j.range[0] < j.range[1])
-      if j.type == S.JNT_FREE:
-        limited = 0
-      if limited and j.range[1] - j.range[0] < 2.0 * j.margin:
-        # both limit rows of the joint could be active at once; the engine keeps one row per joint
-        raise NotImplementedError(
-          f"joint '{j.name}': range narrower than twice its margin (both limits active at once) is not supported")
-      A["jnt_limited"].append(limited)
-      A["jnt_range"].append(j.range)
-      A["jnt_solref"].append(j.solref_limit)
-      A["jnt_solimp"].append(j.solimp_limit)
-      A["jnt_margin"].append(j.margin)
-      A["jnt_stiffness"].append(j.stiffness)
-      if j.type == S.JNT_FREE:
-        n_q, n_v = 7, 6
-        qpos0.extend([*b.pos, *(b.quat / np.linalg.norm(b.quat))])
-      elif j.type == S.JNT_BALL:
-        raise NotImplementedError("ball joints are outside the hot-path feature subset")
-      else:
-        n_q, n_v = 1, 1
-        qpos0.append(j.ref)
-      for k in range(n_v):
-        A["dof_bodyid"].append(b.id)
-        A["dof_jntid"].append(jid)
-        A["dof_parentid"].append(par_dof)
-        A["dof_armature"].append(j.armature)
-        A["dof_damping"].append(j.damping)
-        A["dof_frictionloss"].append(j.frictionloss)
-        par_dof = nv + k
-      nq += n_q
-      nv += n_v
-      ndof_b += n_v
-      jid += 1
-    if ndof_b:
-      dof_last_of_body[b.id] = nv - 1
-    A["body_dofnum"].append(ndof_b)
-    for g in b.geoms:
-      g.id = gid
-      names["geom"].append(g.name)
-      A["geom_type"].append(g.type)
-      A["geom_bodyid"].append(b.id)
-      dataid, size, rbound = -1, g.size, _rbound(g.type, g.size)
-      colliding = True
-      if g.type == S.GEOM_MESH:
-        # A mesh collides (through its convex hull) when it has collision bits and vertex data; a mesh whose
-        # file cannot be read stays what it always was here: a visual.
-        colliding = False
-        mesh = spec.meshes.get(g.mesh) if g.mesh else None
-        if mesh is not None and (g.contype or g.conaffinity):
-          try:
-            v = mesh.load()
-          except OSError as e:
-            raise FileNotFoundError(f"geom '{g.name}': mesh '{g.mesh}' has collision bits but its file is unreadable ({e})") from None
-          if g.mesh not in mesh_ids:
-            mesh_ids[g.mesh] = len(mesh_ids)
-            A["mesh_vertadr"].append(sum(A["mesh_vertnum"]))
-            A["mesh_vertnum"].append(len(v))
-            A["mesh_vert"].extend(v.tolist())
-          dataid, colliding = mesh_ids[g.mesh], True
-          size = np.abs(v).max(axis=0)
-          rbound = float(np.linalg.norm(v, axis=1).max())
-      elif g.type == S.GEOM_HFIELD:
-        hf = spec.hfields.get(g.hfield) if g.hfield else None
-        if hf is None:
-          raise ValueError(f"geom '{g.name}': hfield asset '{g.hfield}' not found")
-        if g.hfield not in hfield_ids:
-          hfield_ids[g.hfield] = len(hfield_ids)
-          A["hfield_adr"].append(len(A["hfield_data"]))
-          A["hfield_nrow"].append(hf.nrow)
-          A["hfield_ncol"].append(hf.ncol)
-          A["hfield_size"].append(hf.size)
-          A["hfield_data"].extend(np.asarray(hf.userdata, dtype=float).reshape(-1).tolist())
-        dataid = hfield_ids[g.hfield]
-        size = np.array(hf.size[:3], dtype=float)
-        rbound = float(np.sqrt(hf.size[0] ** 2 + hf.size[1] ** 2 + max(hf.size[2], hf.size[3]) ** 2))
-      A["geom_dataid"].append(dataid)
-      A["geom_contype"].append(g.contype if colliding else 0)
-      A["geom_conaffinity"].append(g.conaffinity if colliding else 0)
-      A["geom_condim"].append(g.condim)
-      A["geom_priority"].append(g.priority)
-      A["geom_size"].append(size)
-      A["geom_pos"].append(g.pos)
-      A["geom_quat"].append(g.quat / np.linalg.norm(g.quat))
-      A["geom_friction"].append(g.friction)
-      A["geom_solref"].append(g.solref)
-      A["geom_solimp"].append(g.solimp)
-      A["geom_solmix"].append(g.solmix)
-      A["geom_margin"].append(g.margin)
-      A["geom_gap"].append(g.gap)
-      A["geom_rbound"].append(rbound)
-      A["geom_rgba"].append(g.rgba)
-      gid += 1
-    for s in b.sites:
-      s.id = sid
-      names["site"].append(s.name)
-      A["site_bodyid"].append(b.id)
-      A["site_pos"].append(s.pos)
-      A["site_quat"].append(s.quat / np.linalg.norm(s.quat))
-      sid += 1
-  njnt, ngeom, nsite = jid, gid, sid
 
-  parent = np.array(A["body_parentid"], dtype=np.int32)
-  dofnum = np.array(A["body_dofnum"], dtype=np.int32)
-  weld = np.zeros(nbody, dtype=np.int32)
-  root = np.zeros(nbody, dtype=np.int32)
-  for i in range(1, nbody):
+def _body(spec: S.Spec, b: S.Body, A: dict, names: dict) -> None:
+  """Frame and inertial of body ``b`` (from its geoms when it has no ``<inertial>``)."""
+  b.id = len(names["body"])
+  names["body"].append(b.name)
+  A["body_parentid"].append(b.parent.id if b.parent is not None else 0)
+  A["body_pos"].append(b.pos)
+  A["body_quat"].append(b.quat / np.linalg.norm(b.quat))
+  if b.mass is not None:
+    ipos, iquat, mass, inertia = b.ipos, b.iquat, b.mass, b.inertia
+  else:
+    ipos, iquat, mass, inertia = _body_inertial_from_geoms(b, spec.meshes)
+  A["body_ipos"].append(ipos)
+  A["body_iquat"].append(iquat / np.linalg.norm(iquat))
+  A["body_mass"].append(mass)
+  A["body_inertia"].append(inertia)
+
+
+def _joints(spec: S.Spec, b: S.Body, A: dict, names: dict) -> None:
+  """Joints and dofs of body ``b``."""
+  qpos0, nv0 = A["qpos0"], len(A["dof_bodyid"])
+  # dof chain parent: last dof of the nearest ancestor that has dofs
+  anc = b.parent
+  while anc is not None and not A["body_dofnum"][anc.id]:
+    anc = anc.parent
+  par_dof = -1 if anc is None else A["body_dofadr"][anc.id] + A["body_dofnum"][anc.id] - 1
+  A["body_jntadr"].append(len(names["joint"]) if b.joints else -1)
+  A["body_jntnum"].append(len(b.joints))
+  A["body_dofadr"].append(nv0 if b.joints else -1)
+  for j in b.joints:
+    j.id = len(names["joint"])
+    names["joint"].append(j.name)
+    A["jnt_type"].append(j.type)
+    A["jnt_qposadr"].append(len(qpos0))
+    A["jnt_dofadr"].append(len(A["dof_bodyid"]))
+    A["jnt_bodyid"].append(b.id)
+    A["jnt_pos"].append(j.pos)
+    A["jnt_axis"].append(j.axis)
+    limited = j.limited
+    if limited == 2:
+      limited = int(spec.autolimits and j.range[0] < j.range[1])
+    if j.type == S.JNT_FREE:
+      limited = 0
+    if limited and j.range[1] - j.range[0] < 2.0 * j.margin:
+      # both limit rows of the joint could be active at once; the engine keeps one row per joint
+      raise NotImplementedError(
+        f"joint '{j.name}': range narrower than twice its margin (both limits active at once) is not supported")
+    A["jnt_limited"].append(limited)
+    A["jnt_range"].append(j.range)
+    A["jnt_solref"].append(j.solref_limit)
+    A["jnt_solimp"].append(j.solimp_limit)
+    A["jnt_margin"].append(j.margin)
+    A["jnt_stiffness"].append(j.stiffness)
+    if j.type == S.JNT_BALL:
+      raise NotImplementedError("ball joints are outside the hot-path feature subset")
+    qpos0.extend([*b.pos, *(b.quat / np.linalg.norm(b.quat))] if j.type == S.JNT_FREE else [j.ref])
+    for _ in range(JOINT_WIDTH[j.type][1]):
+      A["dof_parentid"].append(par_dof)
+      par_dof = len(A["dof_bodyid"])
+      A["dof_bodyid"].append(b.id)
+      A["dof_jntid"].append(j.id)
+      A["dof_armature"].append(j.armature)
+      A["dof_damping"].append(j.damping)
+      A["dof_frictionloss"].append(j.frictionloss)
+  A["body_dofnum"].append(len(A["dof_bodyid"]) - nv0)
+
+
+def _geoms(spec: S.Spec, b: S.Body, A: dict, names: dict, mesh_ids: dict, hfield_ids: dict) -> None:
+  """Geoms of body ``b``; the first geom to use a mesh or height field adds the asset's data."""
+  for g in b.geoms:
+    g.id = len(names["geom"])
+    names["geom"].append(g.name)
+    A["geom_type"].append(g.type)
+    A["geom_bodyid"].append(b.id)
+    dataid, size, rbound = -1, g.size, _rbound(g.type, g.size)
+    colliding = True
+    if g.type == S.GEOM_MESH:
+      # A mesh collides (through its convex hull) when it has collision bits and vertex data; a mesh whose
+      # file cannot be read stays what it always was here: a visual.
+      colliding = False
+      mesh = spec.meshes.get(g.mesh) if g.mesh else None
+      if mesh is not None and (g.contype or g.conaffinity):
+        try:
+          v = mesh.load()
+        except OSError as e:
+          raise FileNotFoundError(f"geom '{g.name}': mesh '{g.mesh}' has collision bits but its file is unreadable ({e})") from None
+        if g.mesh not in mesh_ids:
+          mesh_ids[g.mesh] = len(mesh_ids)
+          A["mesh_vertadr"].append(sum(A["mesh_vertnum"]))
+          A["mesh_vertnum"].append(len(v))
+          A["mesh_vert"].extend(v.tolist())
+        dataid, colliding = mesh_ids[g.mesh], True
+        size = np.abs(v).max(axis=0)
+        rbound = float(np.linalg.norm(v, axis=1).max())
+    elif g.type == S.GEOM_HFIELD:
+      hf = spec.hfields.get(g.hfield) if g.hfield else None
+      if hf is None:
+        raise ValueError(f"geom '{g.name}': hfield asset '{g.hfield}' not found")
+      if g.hfield not in hfield_ids:
+        hfield_ids[g.hfield] = len(hfield_ids)
+        A["hfield_adr"].append(len(A["hfield_data"]))
+        A["hfield_nrow"].append(hf.nrow)
+        A["hfield_ncol"].append(hf.ncol)
+        A["hfield_size"].append(hf.size)
+        A["hfield_data"].extend(np.asarray(hf.userdata, dtype=float).reshape(-1).tolist())
+      dataid = hfield_ids[g.hfield]
+      size = np.array(hf.size[:3], dtype=float)
+      rbound = float(np.sqrt(hf.size[0] ** 2 + hf.size[1] ** 2 + max(hf.size[2], hf.size[3]) ** 2))
+    A["geom_dataid"].append(dataid)
+    A["geom_contype"].append(g.contype if colliding else 0)
+    A["geom_conaffinity"].append(g.conaffinity if colliding else 0)
+    A["geom_condim"].append(g.condim)
+    A["geom_priority"].append(g.priority)
+    A["geom_size"].append(size)
+    A["geom_pos"].append(g.pos)
+    A["geom_quat"].append(g.quat / np.linalg.norm(g.quat))
+    A["geom_friction"].append(g.friction)
+    A["geom_solref"].append(g.solref)
+    A["geom_solimp"].append(g.solimp)
+    A["geom_solmix"].append(g.solmix)
+    A["geom_margin"].append(g.margin)
+    A["geom_gap"].append(g.gap)
+    A["geom_rbound"].append(rbound)
+    A["geom_rgba"].append(g.rgba)
+
+
+def _sites(b: S.Body, A: dict, names: dict) -> None:
+  for s in b.sites:
+    s.id = len(names["site"])
+    names["site"].append(s.name)
+    A["site_bodyid"].append(b.id)
+    A["site_pos"].append(s.pos)
+    A["site_quat"].append(s.quat / np.linalg.norm(s.quat))
+
+
+def _weld_and_root(A: dict) -> None:
+  """``body_weldid``: the nearest body at or above each body that has dofs (0: welded to the world);
+  ``body_rootid``: the child of the world body it hangs from."""
+  parent, dofnum = A["body_parentid"], A["body_dofnum"]
+  weld = np.zeros(len(parent), dtype=np.int32)
+  root = np.zeros(len(parent), dtype=np.int32)
+  for i in range(1, len(parent)):
     weld[i] = i if dofnum[i] > 0 else weld[parent[i]]
     root[i] = i if parent[i] == 0 else root[parent[i]]
-  A["body_weldid"] = weld
-  A["body_rootid"] = root
+  A["body_weldid"], A["body_rootid"] = weld, root
 
-  # ---- actuators -------------------------------------------------------------------------
+
+def _actuators(spec: S.Spec, A: dict, names: dict) -> None:
   for k, a in enumerate(spec.actuators):
     a.id = k
     names["actuator"].append(a.name)
@@ -587,9 +590,9 @@ def compile_spec(spec: S.Spec) -> Model:
     A["actuator_gainprm"].append(np.array(a.gainprm, dtype=float))
     A["actuator_biasprm"].append(np.array(a.biasprm, dtype=float))
     A["actuator_gear"].append(a.gear)
-  nu = len(spec.actuators)
 
-  # ---- sensors (contact sensors only) ----------------------------------------------------
+
+def _contact_sensors(spec: S.Spec, A: dict, names: dict) -> None:
   adr = 0
   kind_of = {S.OBJ_BODY: "body", S.OBJ_XBODY: "body", S.OBJ_GEOM: "geom", S.OBJ_SITE: "site"}
   for k, sn in enumerate(spec.sensors):
@@ -616,15 +619,17 @@ def compile_spec(spec: S.Spec) -> Model:
     A["sensor_adr"].append(adr)
     A["sensor_dim"].append(dim)
     adr += dim
-  nsensordata = adr
 
-  # ---- candidate collision pairs (mj_collision's static filters) -------------------------
+
+def _collision_pairs(spec: S.Spec, A: dict, names: dict) -> None:
+  """Candidate collision pairs (mj_collision's static filters), and the static grid that replaces the pairs of
+  static geoms when there are more than STATIC_GRID_THRESHOLD of them."""
   excl = set()
   for b1, b2 in spec.excludes:
     i1, i2 = names["body"].index(b1), names["body"].index(b2)
     excl.add((min(i1, i2), max(i1, i2)))
-  gtype = A["geom_type"]
-  gbody = A["geom_bodyid"]
+  gtype, gbody, weld, parent = A["geom_type"], A["geom_bodyid"], A["body_weldid"], A["body_parentid"]
+  ngeom = len(gtype)
   # static collision geoms: on a body welded to the world, not a plane, with any collision bit
   static = [g for g in range(ngeom)
             if weld[gbody[g]] == 0 and gtype[g] not in (S.GEOM_PLANE, S.GEOM_MESH, S.GEOM_HFIELD)
@@ -667,37 +672,32 @@ def compile_spec(spec: S.Spec) -> Model:
   A["pair_geom2"] = [p[1] for p in pairs]
   _build_static_grid(A, static if use_grid else [], weld, gbody, gtype, ngeom)
 
-  # features the engine does not implement must fail here, not silently change the physics
-  used = {g for p in pairs for g in p}
+
+def _refuse_unsupported(A: dict, names: dict) -> None:
+  """Features the engine does not implement must fail here, not silently change the physics."""
+  used = {g for p in zip(A["pair_geom1"], A["pair_geom2"]) for g in p}
   for g in used:
     if A["geom_condim"][g] not in (1, 3):
       raise NotImplementedError(
         f"geom '{names['geom'][g]}': condim {A['geom_condim'][g]} (torsional/rolling friction) is not implemented")
   if any(f != 0 for f in A["dof_frictionloss"]):
     raise NotImplementedError("joint frictionloss (dry-friction constraint rows) is not implemented")
-  A["qpos0"] = qpos0
-  m = Model()
-  shapes = {
-    "body_pos": 3, "body_quat": 4, "body_ipos": 3, "body_iquat": 4, "body_inertia": 3,
-    "jnt_pos": 3, "jnt_axis": 3, "jnt_range": 2, "jnt_solref": 2, "jnt_solimp": 5,
-    "geom_size": 3, "geom_pos": 3, "geom_quat": 4, "geom_friction": 3, "geom_solref": 2,
-    "geom_solimp": 5, "geom_rgba": 4, "site_pos": 3, "site_quat": 4,
-    "actuator_gainprm": 10, "actuator_biasprm": 10, "actuator_ctrlrange": 2,
-    "actuator_forcerange": 2, "sensor_intprm": 3, "body_invweight0": 2, "static_cell0": 2,
-    "mesh_vert": 3, "hfield_size": 4,
-  }
-  for k, dt in MODEL_ARRAYS:
-    if k in ("body_subtreemass", "body_invweight0", "dof_invweight0"):
-      continue
-    arr = np.array(A[k], dtype=np.float64 if dt == "f" else np.int32)
-    if k in shapes:
-      arr = arr.reshape(-1, shapes[k])
-    m.arrays[k] = np.ascontiguousarray(arr)
+  if len(A["dof_bodyid"]) > 64 or len(names["body"]) > 64:
+    raise NotImplementedError("hot path supports nv <= 64 and nbody <= 64 (dof/body bitmasks)")
+
+
+def _pack(spec: S.Spec, A: dict, names: dict) -> Model:
+  """The arrays of MODEL_ARRAYS that the stages built, the sizes and the options, as a Model."""
   o = spec.option
-  m.opt_gravity = np.array(o.gravity, dtype=float)
+  m = Model(names=names, opt_gravity=np.array(o.gravity, dtype=float))
+  for a in MODEL_ARRAYS:
+    if not a.set_const:
+      arr = np.array(A[a.name], dtype=a.dtype)
+      m.arrays[a.name] = np.ascontiguousarray(arr if a.width is None else arr.reshape(-1, a.width))
   scal = dict(
-    nq=nq, nv=nv, nu=nu, nbody=nbody, njnt=njnt, ngeom=ngeom, nsite=nsite,
-    nsensor=len(spec.sensors), nsensordata=nsensordata, npair=len(pairs), nstatic=len(A["static_geom"]),
+    nq=len(A["qpos0"]), nv=len(A["dof_bodyid"]), nu=len(names["actuator"]), nbody=len(names["body"]),
+    njnt=len(names["joint"]), ngeom=len(names["geom"]), nsite=len(names["site"]), nsensor=len(names["sensor"]),
+    nsensordata=sum(A["sensor_dim"]), npair=len(A["pair_geom1"]), nstatic=len(A["static_geom"]),
     opt_integrator=o.integrator, opt_cone=o.cone, opt_solver=o.solver,
     opt_iterations=o.iterations, opt_ls_iterations=o.ls_iterations,
     opt_timestep=o.timestep, opt_tolerance=o.tolerance, opt_ls_tolerance=o.ls_tolerance,
@@ -705,23 +705,23 @@ def compile_spec(spec: S.Spec) -> Model:
   )
   for k, v in scal.items():
     m.arrays[k] = np.array(v, dtype=np.int32 if k in MODEL_SCALARS_I else np.float64)
-  m.names = names
-  if nv > 64 or nbody > 64:
-    raise NotImplementedError("hot path supports nv <= 64 and nbody <= 64 (dof/body bitmasks)")
-  _set_const(m)
+  return m
+
+
+def _keyframes(spec: S.Spec, m: Model) -> None:
+  nq, nv, nu = int(m.nq), int(m.nv), int(m.nu)
   for k in spec.keys:
     qp = k.qpos if k.qpos is not None else m.qpos0
     qv, ct = k.qvel, k.ctrl
     if k.scope is not None and len(qp) != nq:
       # a key of an attached child: its values sit at the child's joints / actuators, defaults elsewhere
-      jn, an = names["joint"], names["actuator"]
+      jn, an = m.names["joint"], m.names["actuator"]
       full_q, full_v, full_c = np.array(m.qpos0, dtype=float), np.zeros(nv), np.zeros(nu)
-      width = {0: (7, 6), 1: (4, 3), 2: (1, 1), 3: (1, 1)}
       iq = iv = 0
       for name in k.scope[0]:
         j = jn.index(name)
-        wq, wv = width[int(A["jnt_type"][j])]
-        qa, va = int(A["jnt_qposadr"][j]), int(A["jnt_dofadr"][j])
+        wq, wv = JOINT_WIDTH[int(m.jnt_type[j])]
+        qa, va = int(m.jnt_qposadr[j]), int(m.jnt_dofadr[j])
         if iq + wq <= len(qp):
           full_q[qa:qa + wq] = np.asarray(qp, dtype=float)[iq:iq + wq]
         if qv is not None and iv + wv <= len(qv):
@@ -739,7 +739,6 @@ def compile_spec(spec: S.Spec) -> Model:
       qvel=np.zeros(nv) if qv is None else np.array(qv, dtype=float),
       ctrl=np.zeros(nu) if ct is None or len(ct) != nu else np.array(ct, float),
     )
-  return m
 
 
 # ---------------------------------------------------------------------------------------

@@ -9,7 +9,7 @@ from pathlib import Path
 
 import numpy as np
 
-from mjlab_b200.compiler.compile import MODEL_ARRAYS, MODEL_SCALARS_F, MODEL_SCALARS_I, fill_asset_defaults
+from mjlab_b200.compiler.compile import MODEL_ARRAYS, MODEL_SCALARS_F, MODEL_SCALARS_I
 
 LIB_PATH = Path(os.environ.get("B2SIM_LIB") or Path(__file__).resolve().parents[1] / "csrc" / "libb2sim.so")
 
@@ -80,8 +80,7 @@ START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive 
 def make_model_desc(model):
   """Pack a compiled Model into a B2ModelDesc. Returns (desc, keepalive)."""
   keep = []
-  names = [n for n, _ in MODEL_ARRAYS] + MODEL_SCALARS_I + MODEL_SCALARS_F
-  fill_asset_defaults(model.arrays)
+  names = [a.name for a in MODEL_ARRAYS] + MODEL_SCALARS_I + MODEL_SCALARS_F
   arrs = (B2Array * len(names))()
   for i, n in enumerate(names):
     a = np.asarray(model.arrays[n])

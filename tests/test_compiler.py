@@ -180,14 +180,13 @@ def test_unsupported_features_fail_loudly():
 
 def test_compiled_blobs_are_reproducible_from_the_reference_xml(monkeypatch):
   """The model blobs shipped in asset_zoo/compiled (what every GPU test and the bench load) are exactly what the
-  compiler produces today from the reference's MJCF (as installed under oracle/_ref): arrays, names and keyframes,
-  bit for bit."""
+  compiler produces today from the reference's MJCF (as installed under oracle/_ref): arrays (dtype, shape and
+  values), names and keyframes, bit for bit."""
   import sys
 
   import refload
   from mjlab_b200 import asset_zoo
-  from mjlab_b200.asset_zoo import g1, go1, load_compiled, reference_xml
-  from mjlab_b200.asset_zoo.scene import compile_scene
+  from mjlab_b200.asset_zoo import COMPILED_DIR, load_compiled, reference_xml
 
   monkeypatch.setattr(asset_zoo, "_REF_ZOO", refload.REF / "mjlab" / "asset_zoo" / "robots")
   try:
@@ -197,18 +196,15 @@ def test_compiled_blobs_are_reproducible_from_the_reference_xml(monkeypatch):
   sys.path.insert(0, str(__import__("pathlib").Path(__file__).resolve().parents[1] / "tools"))
   import compile_assets as ca
 
-  fresh = {
-    "g1_flat": compile_scene(g1.robot_cfg(g1_xml, g1.velocity_sensors()), ca.TASK),
-    "g1_tracking_flat": compile_scene(g1.robot_cfg(g1_xml, g1.tracking_sensors()), ca.TASK),
-    "go1_flat": compile_scene(go1.robot_cfg(go1_xml, go1.velocity_sensors()), ca.TASK),
-    "go1_hf_small": compile_scene(go1.robot_cfg(go1_xml, go1.velocity_sensors()), ca.TASK, ca.SMALL_HF),
-  }
+  fresh = ca.compile_all(g1_xml, go1_xml)
+  assert sorted(fresh) == sorted(p.stem for p in COMPILED_DIR.glob("*.npz"))
   for name, m in fresh.items():
     old = load_compiled(name)
     assert old.names == m.names, name
     assert set(old.arrays) == set(m.arrays), (name, set(old.arrays) ^ set(m.arrays))
     for k in old.arrays:
-      assert np.array_equal(np.asarray(old.arrays[k]), np.asarray(m.arrays[k])), (name, k)
+      a, b = np.asarray(old.arrays[k]), np.asarray(m.arrays[k])
+      assert a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a, b), (name, k, a.dtype, b.dtype)
     for k in old.keys:
       for f in ("qpos", "qvel", "ctrl"):
         assert np.array_equal(old.keys[k][f], m.keys[k][f]), (name, k, f)

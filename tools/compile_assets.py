@@ -31,10 +31,9 @@ SMALL_HF = RoughTerrainCfg(num_rows=2, num_cols=4, border_width=2.0, seed=5, dif
 FULL_HF = RoughTerrainCfg(seed=0, sub_terrains=FULL_SUB_TERRAINS)
 
 
-def main():
-  COMPILED_DIR.mkdir(exist_ok=True)
-  g1_xml, go1_xml = reference_xml("g1"), reference_xml("go1")
-  out = {
+def compile_all(g1_xml, go1_xml) -> dict:
+  """Every shipped blob's model, by blob name."""
+  return {
     "g1_flat": compile_scene(g1.robot_cfg(g1_xml, g1.velocity_sensors()), TASK),
     "g1_tracking_flat": compile_scene(g1.robot_cfg(g1_xml, g1.tracking_sensors()), TASK),
     "go1_flat": compile_scene(go1.robot_cfg(go1_xml, go1.velocity_sensors()), TASK),
@@ -43,7 +42,11 @@ def main():
     "go1_hf_small": compile_scene(go1.robot_cfg(go1_xml, go1.velocity_sensors()), TASK, SMALL_HF),
     "go1_rough_hf": compile_scene(go1.robot_cfg(go1_xml, go1.velocity_sensors()), TASK, FULL_HF),
   }
-  for name, m in out.items():
+
+
+def main():
+  COMPILED_DIR.mkdir(exist_ok=True)
+  for name, m in compile_all(reference_xml("g1"), reference_xml("go1")).items():
     m.save(COMPILED_DIR / f"{name}.npz")
     print(
       f"{name}: nq={int(m.nq)} nv={int(m.nv)} nu={int(m.nu)} nbody={int(m.nbody)} "
