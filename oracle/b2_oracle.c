@@ -66,6 +66,41 @@ enum { EFC_LIMIT = 3, EFC_FRICTIONLESS = 4, EFC_PYRAMIDAL = 5 };
   X(actuator_ctrlrange) X(actuator_forcerange) X(actuator_gear) X(qpos0)                        \
   X(mesh_vert) X(hfield_size) X(hfield_data)
 
+/* scalars read from the model description: (member, model array, element) */
+#define MODEL_SCALAR(X)                                                                         \
+  X(nq, nq, 0) X(nv, nv, 0) X(nu, nu, 0) X(nbody, nbody, 0) X(njnt, njnt, 0) X(ngeom, ngeom, 0)  \
+  X(nsite, nsite, 0) X(nsensor, nsensor, 0) X(nsensordata, nsensordata, 0) X(npair, npair, 0)    \
+  X(integrator, opt_integrator, 0) X(cone, opt_cone, 0) X(solver, opt_solver, 0)                \
+  X(iterations, opt_iterations, 0) X(ls_iterations, opt_ls_iterations, 0)                       \
+  X(timestep, opt_timestep, 0) X(tolerance, opt_tolerance, 0) X(ls_tolerance, opt_ls_tolerance, 0) \
+  X(impratio, opt_impratio, 0) X(meaninertia, stat_meaninertia, 0) X(nstatic, nstatic, 0)       \
+  X(grid_x0, grid_params, 0) X(grid_y0, grid_params, 1) X(grid_cell, grid_params, 2)            \
+  X(grid_nx, grid_params, 3) X(grid_ny, grid_params, 4)
+
+/* options b2o_set_option accepts: (member, type); the option's name is the member's */
+#define OPTIONS(X)                                                                              \
+  X(iterations, int) X(ls_iterations, int) X(tolerance, real) X(ls_tolerance, real)            \
+  X(timestep, real) X(integrator, int)
+
+/* Data fields, [nworld][row length] each: (name, row length).  A field whose rows are empty still gets
+ * one element per world. */
+#define DATA_REAL(X)                                                                            \
+  X(qpos, nq) X(qvel, nv) X(qacc, nv) X(qacc_warmstart, nv) X(ctrl, nu) X(qfrc_applied, nv)      \
+  X(xfrc_applied, 6*nbody) X(xpos, 3*nbody) X(xquat, 4*nbody) X(xmat, 9*nbody)                 \
+  X(xipos, 3*nbody) X(ximat, 9*nbody) X(subtree_com, 3*nbody) X(cinert, 10*nbody) X(cdof, 6*nv) \
+  X(cdof_dot, 6*nv) X(cvel, 6*nbody) X(xanchor, 3*njnt) X(xaxis, 3*njnt) X(geom_xpos, 3*ngeom)  \
+  X(geom_xmat, 9*ngeom) X(site_xpos, 3*nsite) X(site_xmat, 9*nsite) X(qM, nv*nv) X(qL, nv*nv)   \
+  X(qfrc_bias, nv) X(qfrc_passive, nv) X(qfrc_actuator, nv) X(actuator_force, nu)              \
+  X(qfrc_smooth, nv) X(qacc_smooth, nv) X(qfrc_constraint, nv) X(sensordata, nsensordata)      \
+  X(time, 1) X(contact_dist, maxcon) X(contact_pos, 3*maxcon) X(contact_frame, 9*maxcon)       \
+  X(contact_friction, 5*maxcon) X(contact_solref, 2*maxcon) X(contact_solimp, 5*maxcon)        \
+  X(contact_includemargin, maxcon) X(contact_force, 3*maxcon) X(efc_J, njmax*nv)               \
+  X(efc_pos, njmax) X(efc_margin, njmax) X(efc_D, njmax) X(efc_R, njmax) X(efc_aref, njmax)    \
+  X(efc_vel, njmax) X(efc_force, njmax) X(solver_cost, 1)
+#define DATA_INT(X)                                                                             \
+  X(ncon, 1) X(nefc, 1) X(contact_dim, maxcon) X(contact_geom, 2*maxcon) X(contact_efc, maxcon) \
+  X(efc_type, njmax) X(efc_id, njmax) X(solver_niter, 1) X(overflow, 1)
+
 typedef struct { real* p; int n; int stride; } MF; /* stride 0 = shared by all worlds */
 
 typedef struct B2Oracle {
@@ -80,11 +115,13 @@ typedef struct B2Oracle {
 #define X(n) MF n;
   MODEL_REAL(X)
 #undef X
-  /* data: name table */
-  int nfield;
-  struct { const char* name; real* p; int rowlen; } field[64];
-  int nifield;
-  struct { const char* name; int* p; int rowlen; } ifield[16];
+  struct {
+#define R(n, len) struct { real* p; int rowlen; } n;
+#define I(n, len) struct { int* p; int rowlen; } n;
+    DATA_REAL(R) DATA_INT(I)
+#undef R
+#undef I
+  } data;
 } B2Oracle;
 
 static const B2Array* find_arr(const B2ModelDesc* d, const char* name) {
@@ -93,13 +130,10 @@ static const B2Array* find_arr(const B2ModelDesc* d, const char* name) {
   fprintf(stderr, "b2_oracle: model array '%s' missing\n", name);
   abort();
 }
-static int get_i(const B2ModelDesc* d, const char* name) {
+static double get_scalar(const B2ModelDesc* d, const char* name, int k) {
   const B2Array* a = find_arr(d, name);
-  return a->dtype == B2_I32 ? ((const int32_t*)a->data)[0] : (int)((const double*)a->data)[0];
-}
-static double get_f(const B2ModelDesc* d, const char* name) {
-  const B2Array* a = find_arr(d, name);
-  return a->dtype == B2_I32 ? ((const int32_t*)a->data)[0] : ((const double*)a->data)[0];
+  if (k >= a->n) { fprintf(stderr, "b2_oracle: model array '%s' has no element %d\n", name, k); abort(); }
+  return a->dtype == B2_I32 ? ((const int32_t*)a->data)[k] : ((const double*)a->data)[k];
 }
 static int* dup_i(const B2ModelDesc* d, const char* name) {
   const B2Array* a = find_arr(d, name);
@@ -116,19 +150,6 @@ static MF dup_f(const B2ModelDesc* d, const char* name) {
   return m;
 }
 #define M_(o, name, w) ((o)->name.p + (size_t)(w) * (o)->name.stride)
-
-static real* add_field(B2Oracle* o, const char* name, int rowlen) {
-  real* p = (real*)calloc((size_t)o->nworld * (rowlen ? rowlen : 1), sizeof(real));
-  o->field[o->nfield].name = name; o->field[o->nfield].p = p; o->field[o->nfield].rowlen = rowlen;
-  o->nfield++;
-  return p;
-}
-static int* add_ifield(B2Oracle* o, const char* name, int rowlen) {
-  int* p = (int*)calloc((size_t)o->nworld * (rowlen ? rowlen : 1), sizeof(int));
-  o->ifield[o->nifield].name = name; o->ifield[o->nifield].p = p; o->ifield[o->nifield].rowlen = rowlen;
-  o->nifield++;
-  return p;
-}
 
 /* ---------------------------------------------------------------------------------------------
  * small math (MuJoCo engine_util_blas.c / engine_util_spatial.c conventions)
@@ -255,45 +276,18 @@ static void chol_solve(const real* L, int n, real* x) { /* x <- (L L')^-1 x */
  * ------------------------------------------------------------------------------------------- */
 typedef struct W {
   const B2Oracle* o; int w;
-  real *qpos, *qvel, *qacc, *qacc_warmstart, *ctrl, *qfrc_applied, *xfrc_applied;
-  real *xpos, *xquat, *xmat, *xipos, *ximat, *subtree_com, *cinert, *cdof, *cdof_dot, *cvel;
-  real *xanchor, *xaxis, *geom_xpos, *geom_xmat, *site_xpos, *site_xmat;
-  real *qM, *qL, *qfrc_bias, *qfrc_passive, *qfrc_actuator, *actuator_force, *qfrc_smooth;
-  real *qacc_smooth, *qfrc_constraint, *sensordata, *time;
-  real *contact_dist, *contact_pos, *contact_frame, *contact_friction, *contact_solref;
-  real *contact_solimp, *contact_includemargin, *contact_force;
-  real *efc_J, *efc_pos, *efc_margin, *efc_D, *efc_R, *efc_aref, *efc_vel, *efc_force;
-  real *solver_cost;
-  int *ncon, *nefc, *contact_dim, *contact_geom, *contact_efc, *efc_type, *efc_id, *solver_niter;
-  int *overflow;
+#define R(n, len) real* n;
+#define I(n, len) int* n;
+  DATA_REAL(R) DATA_INT(I)
+#undef R
+#undef I
 } W;
 
-static real* F(const B2Oracle* o, const char* name, int w) {
-  for (int i = 0; i < o->nfield; i++)
-    if (!strcmp(o->field[i].name, name)) return o->field[i].p + (size_t)w * o->field[i].rowlen;
-  fprintf(stderr, "b2_oracle: field '%s' missing\n", name); abort();
-}
-static int* FI(const B2Oracle* o, const char* name, int w) {
-  for (int i = 0; i < o->nifield; i++)
-    if (!strcmp(o->ifield[i].name, name)) return o->ifield[i].p + (size_t)w * o->ifield[i].rowlen;
-  fprintf(stderr, "b2_oracle: int field '%s' missing\n", name); abort();
-}
-#define BIND(n) d.n = F(o, #n, w)
-#define BINDI(n) d.n = FI(o, #n, w)
 static W bind(const B2Oracle* o, int w) {
   W d; d.o = o; d.w = w;
-  BIND(qpos); BIND(qvel); BIND(qacc); BIND(qacc_warmstart); BIND(ctrl); BIND(qfrc_applied);
-  BIND(xfrc_applied); BIND(xpos); BIND(xquat); BIND(xmat); BIND(xipos); BIND(ximat);
-  BIND(subtree_com); BIND(cinert); BIND(cdof); BIND(cdof_dot); BIND(cvel); BIND(xanchor);
-  BIND(xaxis); BIND(geom_xpos); BIND(geom_xmat); BIND(site_xpos); BIND(site_xmat); BIND(qM);
-  BIND(qL); BIND(qfrc_bias); BIND(qfrc_passive); BIND(qfrc_actuator); BIND(actuator_force);
-  BIND(qfrc_smooth); BIND(qacc_smooth); BIND(qfrc_constraint); BIND(sensordata); BIND(time);
-  BIND(contact_dist); BIND(contact_pos); BIND(contact_frame); BIND(contact_friction);
-  BIND(contact_solref); BIND(contact_solimp); BIND(contact_includemargin); BIND(contact_force);
-  BIND(efc_J); BIND(efc_pos); BIND(efc_margin); BIND(efc_D); BIND(efc_R); BIND(efc_aref);
-  BIND(efc_vel); BIND(efc_force); BIND(solver_cost);
-  BINDI(ncon); BINDI(nefc); BINDI(contact_dim); BINDI(contact_geom); BINDI(contact_efc);
-  BINDI(efc_type); BINDI(efc_id); BINDI(solver_niter); BINDI(overflow);
+#define X(n, len) d.n = o->data.n.p + (size_t)w * o->data.n.rowlen;
+  DATA_REAL(X) DATA_INT(X)
+#undef X
   return d;
 }
 
@@ -921,8 +915,10 @@ static void collision(W* d) {
     const real* c = d->geom_xpos + 3*g;
     int ix0 = (int)floor((c[0] - rb[g] - o->grid_x0) / o->grid_cell), ix1 = (int)floor((c[0] + rb[g] - o->grid_x0) / o->grid_cell);
     int iy0 = (int)floor((c[1] - rb[g] - o->grid_y0) / o->grid_cell), iy1 = (int)floor((c[1] + rb[g] - o->grid_y0) / o->grid_cell);
-    if (ix0 < 0) ix0 = 0; if (iy0 < 0) iy0 = 0;
-    if (ix1 >= o->grid_nx) ix1 = o->grid_nx - 1; if (iy1 >= o->grid_ny) iy1 = o->grid_ny - 1;
+    if (ix0 < 0) ix0 = 0;
+    if (iy0 < 0) iy0 = 0;
+    if (ix1 >= o->grid_nx) ix1 = o->grid_nx - 1;
+    if (iy1 >= o->grid_ny) iy1 = o->grid_ny - 1;
     int cand[1024], ncand = 0;
     for (int ix = ix0; ix <= ix1; ix++)
       for (int iy = iy0; iy <= iy1; iy++) {
@@ -1484,66 +1480,40 @@ static void world_forward(const B2Oracle* o, int w, int do_step) {
 /* ---------------------------------------------------------------------------------------------
  * public API (test-only)
  * ------------------------------------------------------------------------------------------- */
+static void alloc_data(B2Oracle* o) {
+  /* the names the Data table's row lengths are written in */
+  int nq = o->nq, nv = o->nv, nu = o->nu, nbody = o->nbody, njnt = o->njnt, ngeom = o->ngeom, nsite = o->nsite;
+  int nsensordata = o->nsensordata, maxcon = o->maxcon, njmax = o->njmax;
+#define X(n, len)                                                                               \
+  o->data.n.rowlen = len;                                                                       \
+  o->data.n.p = calloc((size_t)o->nworld * (o->data.n.rowlen ? o->data.n.rowlen : 1), sizeof *o->data.n.p);
+  DATA_REAL(X) DATA_INT(X)
+#undef X
+}
 B2Oracle* b2o_create(const B2ModelDesc* desc, int nworld, int maxcon, int njmax) {
   B2Oracle* o = (B2Oracle*)calloc(1, sizeof(B2Oracle));
-  o->nq = get_i(desc, "nq"); o->nv = get_i(desc, "nv"); o->nu = get_i(desc, "nu");
-  o->nbody = get_i(desc, "nbody"); o->njnt = get_i(desc, "njnt"); o->ngeom = get_i(desc, "ngeom");
-  o->nsite = get_i(desc, "nsite"); o->nsensor = get_i(desc, "nsensor");
-  o->nsensordata = get_i(desc, "nsensordata"); o->npair = get_i(desc, "npair");
-  o->integrator = get_i(desc, "opt_integrator"); o->cone = get_i(desc, "opt_cone");
-  o->solver = get_i(desc, "opt_solver"); o->iterations = get_i(desc, "opt_iterations");
-  o->ls_iterations = get_i(desc, "opt_ls_iterations");
-  o->timestep = (real)get_f(desc, "opt_timestep"); o->tolerance = (real)get_f(desc, "opt_tolerance");
-  o->ls_tolerance = (real)get_f(desc, "opt_ls_tolerance"); o->impratio = (real)get_f(desc, "opt_impratio");
-  o->meaninertia = (real)get_f(desc, "stat_meaninertia");
+#define X(m, arr, k) o->m = get_scalar(desc, #arr, k);
+  MODEL_SCALAR(X)
+#undef X
   for (int k = 0; k < 3; k++) o->gravity[k] = (real)desc->gravity[k];
   o->nworld = nworld; o->maxcon = maxcon > 0 ? maxcon : 64; o->njmax = njmax > 0 ? njmax : 300;
-  o->nstatic = get_i(desc, "nstatic"); o->ndyn = (int)find_arr(desc, "dyn_cgeom")->n;
-  {
-    const B2Array* gp = find_arr(desc, "grid_params");
-    const double* v = (const double*)gp->data;
-    o->grid_x0 = (real)v[0]; o->grid_y0 = (real)v[1]; o->grid_cell = (real)v[2]; o->grid_nx = (int)v[3]; o->grid_ny = (int)v[4];
-  }
+  o->ndyn = (int)find_arr(desc, "dyn_cgeom")->n;
 #define X(n) o->n = dup_i(desc, #n);
   MODEL_INT(X)
 #undef X
 #define X(n) o->n = dup_f(desc, #n);
   MODEL_REAL(X)
 #undef X
-  int nq = o->nq, nv = o->nv, nu = o->nu, nb = o->nbody, nj = o->njnt, ng = o->ngeom, ns = o->nsite;
-  int mc = o->maxcon, jm = o->njmax;
-  add_field(o, "qpos", nq); add_field(o, "qvel", nv); add_field(o, "qacc", nv);
-  add_field(o, "qacc_warmstart", nv); add_field(o, "ctrl", nu); add_field(o, "qfrc_applied", nv);
-  add_field(o, "xfrc_applied", 6*nb); add_field(o, "xpos", 3*nb); add_field(o, "xquat", 4*nb);
-  add_field(o, "xmat", 9*nb); add_field(o, "xipos", 3*nb); add_field(o, "ximat", 9*nb);
-  add_field(o, "subtree_com", 3*nb); add_field(o, "cinert", 10*nb); add_field(o, "cdof", 6*nv);
-  add_field(o, "cdof_dot", 6*nv); add_field(o, "cvel", 6*nb); add_field(o, "xanchor", 3*nj);
-  add_field(o, "xaxis", 3*nj); add_field(o, "geom_xpos", 3*ng); add_field(o, "geom_xmat", 9*ng);
-  add_field(o, "site_xpos", 3*ns); add_field(o, "site_xmat", 9*ns); add_field(o, "qM", nv*nv);
-  add_field(o, "qL", nv*nv); add_field(o, "qfrc_bias", nv); add_field(o, "qfrc_passive", nv);
-  add_field(o, "qfrc_actuator", nv); add_field(o, "actuator_force", nu);
-  add_field(o, "qfrc_smooth", nv); add_field(o, "qacc_smooth", nv);
-  add_field(o, "qfrc_constraint", nv); add_field(o, "sensordata", o->nsensordata);
-  add_field(o, "time", 1);
-  add_field(o, "contact_dist", mc); add_field(o, "contact_pos", 3*mc);
-  add_field(o, "contact_frame", 9*mc); add_field(o, "contact_friction", 5*mc);
-  add_field(o, "contact_solref", 2*mc); add_field(o, "contact_solimp", 5*mc);
-  add_field(o, "contact_includemargin", mc); add_field(o, "contact_force", 3*mc);
-  add_field(o, "efc_J", jm*nv); add_field(o, "efc_pos", jm); add_field(o, "efc_margin", jm);
-  add_field(o, "efc_D", jm); add_field(o, "efc_R", jm); add_field(o, "efc_aref", jm);
-  add_field(o, "efc_vel", jm); add_field(o, "efc_force", jm); add_field(o, "solver_cost", 1);
-  add_ifield(o, "ncon", 1); add_ifield(o, "nefc", 1); add_ifield(o, "contact_dim", mc);
-  add_ifield(o, "contact_geom", 2*mc); add_ifield(o, "contact_efc", mc);
-  add_ifield(o, "efc_type", jm); add_ifield(o, "efc_id", jm); add_ifield(o, "solver_niter", 1);
-  add_ifield(o, "overflow", 1);
+  alloc_data(o);
   for (int w = 0; w < nworld; w++)
-    for (int i = 0; i < nq; i++) F(o, "qpos", w)[i] = o->qpos0.p[i];
+    for (int i = 0; i < o->nq; i++) o->data.qpos.p[(size_t)w*o->nq + i] = o->qpos0.p[i];
   return o;
 }
 void b2o_destroy(B2Oracle* o) {
   if (!o) return;
-  for (int i = 0; i < o->nfield; i++) free(o->field[i].p);
-  for (int i = 0; i < o->nifield; i++) free(o->ifield[i].p);
+#define X(n, len) free(o->data.n.p);
+  DATA_REAL(X) DATA_INT(X)
+#undef X
 #define X(n) free(o->n);
   MODEL_INT(X)
 #undef X
@@ -1553,14 +1523,14 @@ void b2o_destroy(B2Oracle* o) {
   free(o);
 }
 int b2o_real_size(void) { return (int)sizeof(real); }
-void* b2o_field(B2Oracle* o, const char* name, int* rowlen) {
-  for (int i = 0; i < o->nfield; i++)
-    if (!strcmp(o->field[i].name, name)) { *rowlen = o->field[i].rowlen; return o->field[i].p; }
-  return NULL;
-}
-int* b2o_ifield(B2Oracle* o, const char* name, int* rowlen) {
-  for (int i = 0; i < o->nifield; i++)
-    if (!strcmp(o->ifield[i].name, name)) { *rowlen = o->ifield[i].rowlen; return o->ifield[i].p; }
+/* Data field [nworld][*rowlen] by name, of int (*is_int = 1) or real elements; NULL for an unknown name */
+void* b2o_field(B2Oracle* o, const char* name, int* rowlen, int* is_int) {
+#define X(n, len) if (!strcmp(name, #n)) { *rowlen = o->data.n.rowlen; *is_int = 0; return o->data.n.p; }
+  DATA_REAL(X)
+#undef X
+#define X(n, len) if (!strcmp(name, #n)) { *rowlen = o->data.n.rowlen; *is_int = 1; return o->data.n.p; }
+  DATA_INT(X)
+#undef X
   return NULL;
 }
 /* per-world model field (expands it on first use); returns pointer to [nworld][n] reals */
@@ -1578,13 +1548,12 @@ void* b2o_model_field(B2Oracle* o, const char* name, int* n) {
   *n = f->n;
   return f->p;
 }
-void b2o_set_option(B2Oracle* o, const char* key, double v) {
-  if (!strcmp(key, "iterations")) o->iterations = (int)v;
-  else if (!strcmp(key, "ls_iterations")) o->ls_iterations = (int)v;
-  else if (!strcmp(key, "tolerance")) o->tolerance = (real)v;
-  else if (!strcmp(key, "ls_tolerance")) o->ls_tolerance = (real)v;
-  else if (!strcmp(key, "timestep")) o->timestep = (real)v;
-  else if (!strcmp(key, "integrator")) o->integrator = (int)v;
+/* returns 0, or 1 for a name not in OPTIONS */
+int b2o_set_option(B2Oracle* o, const char* key, double v) {
+#define X(n, type) if (!strcmp(key, #n)) { o->n = (type)v; return 0; }
+  OPTIONS(X)
+#undef X
+  return 1;
 }
 static void run(B2Oracle* o, int do_step, int nthread) {
 #ifdef _OPENMP

@@ -50,13 +50,10 @@ def test_objects_rest_on_a_box(geom, z, quat, ncon):
 def _prim_box_box(p1, R1, h1, p2, R2, h2, margin=0.0):
   import ctypes
 
-  from oracle.oracle import build
-  build()
-  L = ctypes.CDLL(str(Path(__file__).parents[1] / "oracle" / "libb2oracle64.so"))
+  from oracle.oracle import load_library
+  L = load_library("f64")
   dp = ctypes.POINTER(ctypes.c_double)
-  L.b2o_prim_box_box.argtypes = [dp] * 6 + [ctypes.c_double, dp]
   out = np.zeros(56)
-  P = lambda a: np.ascontiguousarray(a, dtype=np.float64).ctypes.data_as(dp)
   arrs = [np.ascontiguousarray(np.asarray(a, dtype=np.float64).ravel()) for a in (p1, R1, h1, p2, R2, h2)]
   n = L.b2o_prim_box_box(*[a.ctypes.data_as(dp) for a in arrs], margin, out.ctypes.data_as(dp))
   return n, out[: 7 * n].reshape(n, 7)

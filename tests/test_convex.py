@@ -11,14 +11,13 @@ import numpy as np
 import pytest
 from scipy.spatial import ConvexHull
 
-from oracle.oracle import _DIR, build
+from oracle.oracle import load_library
 
 G_SPHERE, G_CAPSULE, G_BOX, G_MESH = 2, 3, 6, 7
 
 
 def _lib(prec):
-  build()
-  L = ctypes.CDLL(str(_DIR / f"libb2oracle{prec}.so"))
+  L = load_library(f"f{prec}")
   return L, (np.float64 if prec == 64 else np.float32), (ctypes.c_double if prec == 64 else ctypes.c_float)
 
 
@@ -104,7 +103,6 @@ def _call_pair(L, dt, ct, t1, p1, R1, s1, v1, t2, p2, R2, s2, v2, margin, scale)
   out = np.zeros(7, dtype=dt)
   a = lambda x: None if x is None else np.ascontiguousarray(x, dtype=dt)  # noqa: E731
   A = [a(p1), a(R1.reshape(-1)), a(s1), a(v1), a(p2), a(R2.reshape(-1)), a(s2), a(v2)]
-  L.b2o_prim_convex.argtypes = None
   n = L.b2o_prim_convex(ctypes.c_int(t1), _p(A[0]), _p(A[1]), _p(A[2]), _p(A[3]), ctypes.c_int(0 if v1 is None else len(v1)),
                         ctypes.c_int(t2), _p(A[4]), _p(A[5]), _p(A[6]), _p(A[7]), ctypes.c_int(0 if v2 is None else len(v2)),
                         ct(margin), ct(scale), _p(out))

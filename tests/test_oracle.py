@@ -3,14 +3,16 @@
 The reference holds no known-answer tests for this path (SURVEY.md §4, §8c: parity unpinned), so
 these are what pin the restated algorithm."""
 
+import json
+import re
 from pathlib import Path
 
 import numpy as np
 import pytest
 
 from mjlab_b200.compiler import Spec
-from oracle.oracle import Oracle
-from util import load_oracle, make_states, terrain_states
+from oracle.oracle import _DIR, Oracle, load_library
+from util import convex_scene, load_oracle, make_states, terrain_states
 
 GOLDEN = Path(__file__).parent / "golden"
 
@@ -30,6 +32,52 @@ BALL_ON_PLANE = """
     <body name="ball" pos="0 0 0.099"><freejoint/><geom type="sphere" size="0.1" mass="2"/></body>
   </worldbody></mujoco>
 """
+
+
+def test_oracle_field_surface():
+  """Every Data field keeps its name, element type and row length (tests/golden/oracle_fields.json), for a humanoid,
+  a quadruped on a height field and the mesh / height-field scene; an unknown name raises."""
+  from mjlab_b200.asset_zoo import load_compiled
+
+  golden = json.loads((GOLDEN / "oracle_fields.json").read_text())
+  assert sorted(golden) == ["convex_scene", "g1_flat", "go1_rough_hf"]
+  for name, rows in golden.items():
+    m = convex_scene()[0] if name == "convex_scene" else load_compiled(name)
+    for prec in ("f64", "f32"):
+      o = Oracle(m, nworld=2, maxcon=40, njmax=120, precision=prec)
+      got = []
+      for f, _, _ in rows:
+        a = o.field(f)
+        assert a.shape[0] == 2 and a.dtype in (np.int32, o.dtype), (name, f, a.shape, a.dtype)
+        got.append([f, "int" if a.dtype == np.int32 else "real", a.shape[1]])
+      assert got == rows, name
+      with pytest.raises(KeyError):
+        o.field("qpos0")  # a model array, not a Data field
+
+
+def test_oracle_options():
+  m = Spec.from_string(PENDULUM).compile()
+  o = Oracle(m)
+  for k, v in (("iterations", 7), ("ls_iterations", 9), ("tolerance", 1e-6), ("ls_tolerance", 1e-3),
+               ("timestep", 1e-3), ("integrator", 0)):
+    o.set_option(k, v)
+  o.step()
+  assert o.time[0, 0] == 1e-3
+  for k in ("solver", "iteration"):
+    with pytest.raises(ValueError, match=f"'{k}'"):
+      o.set_option(k, 1)
+
+
+def test_oracle_library_binds_every_entry_point():
+  """load_library declares the signature of every b2o_* function b2_oracle.c exports, in both precisions."""
+  src = (_DIR / "b2_oracle.c").read_text()
+  defined = set(re.findall(r"^(?!static)\w[\w \t*]*?\b(b2o_\w+)\s*\(", src, re.M))
+  assert {"b2o_create", "b2o_field", "b2o_set_option", "b2o_prim_hfield"} <= defined
+  for prec in ("f64", "f32"):
+    lib = load_library(prec)
+    for fn in defined:
+      assert hasattr(lib, fn), f"{fn} is defined in b2_oracle.c but not exported by the {prec} library"
+    assert {fn for fn in defined if getattr(lib, fn).argtypes is not None} == defined, prec
 
 
 def test_free_fall_and_momentum():

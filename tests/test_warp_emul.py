@@ -178,10 +178,9 @@ def _rot(rng):
 def test_box_primitives_device_code_matches_oracle(lib):
   """sphere-box, capsule-box and box-box: the CUDA device routines (compiled for the host) against the
   oracle's C routines on random configurations, including far-from-origin placements (fp32 vs fp64)."""
-  from oracle.oracle import build
+  from oracle.oracle import load_library
 
-  build()
-  orc = ctypes.CDLL(str(Path(__file__).parents[1] / "oracle" / "libb2oracle64.so"))
+  orc = load_library("f64")
   dp, fp = ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float)
   rng = np.random.default_rng(11)
   counts = {"sphere": 0, "capsule": 0, "capsule2": 0, "box": 0}
