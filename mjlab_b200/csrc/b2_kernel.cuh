@@ -199,7 +199,7 @@ __device__ unsigned long long g_phase_cycles[32];
 
 // approximate reciprocal (MUFU.RCP): the IEEE-rounded __frcp_rn costs ~13 instructions per call
 __device__ __forceinline__ float b2_rcp(float x) {
-#if defined(B2_HOST_EMULATION) || defined(B2_PRECISE_RCP)
+#ifdef B2_HOST_EMULATION
   return __frcp_rn(x);
 #else
   float r;
@@ -733,7 +733,7 @@ __device__ __noinline__ int hfield_lanes(RawCon* rc, bool hf, float margin, cons
     if (lane >= o) incl += t;
   }
   const int total = __shfl_sync(FULL, incl, 31);
-  PHASE_MARK(21);  // footprints
+  PHASE_MARK(21);  // (hfield: footprints)
   if (total == 0) return 0;
   __syncwarp();
   B2CCon out[B2C_MAXOUT];
@@ -772,7 +772,7 @@ __device__ __noinline__ int hfield_lanes(RawCon* rc, bool hf, float margin, cons
       qn += __popc(km);
       i0 += 32;
       __syncwarp();
-      PHASE_MARK(22);  // cull
+      PHASE_MARK(22);  // (hfield: cull)
     }
     if (qn >= 32 || (i0 >= total && qn > 0)) {
       const int take = min(qn, 32);
@@ -813,7 +813,7 @@ __device__ __noinline__ int hfield_lanes(RawCon* rc, bool hf, float margin, cons
       if (lane < rest) queue[lane] = mv;
       __syncwarp();
       qn = rest;
-      PHASE_MARK(23);  // prisms (GJK / EPA) + merge
+      PHASE_MARK(23);  // (hfield: prisms + merge)
     }
   }
   b2c_hfield_sort(out, order, n);
@@ -1022,7 +1022,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     barphase ^= 1u;
   }
 
-  PHASE_MARK(0);
+  PHASE_MARK(0);  // load(TMA)
   PSYNC();
 
   // Consumer-visible kinematics (poses, cvel, derived velocities) are observable only after the last sub-step
@@ -1160,7 +1160,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   }
   __syncwarp();
 
-  PHASE_MARK(1);
+  PHASE_MARK(1);  // kinematics
   PSYNC();
   REGIONS();
   // geom / site world poses -> global (and shared for collidable geoms)
@@ -1209,7 +1209,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     }
   }
 
-  PHASE_MARK(2);
+  PHASE_MARK(2);  // geom/site poses
   PSYNC();
   REGIONS();
   // ---------------- phase 2: subtree com, spatial inertias, motion vectors -----------------------
@@ -1317,7 +1317,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   }
   __syncwarp();
 
-  PHASE_MARK(3);
+  PHASE_MARK(3);  // com/cinert/cdof
   PSYNC();
   REGIONS();
   // ---------------- phase 3: composite inertias -> joint-space inertia M (packed lower) ----------
@@ -1349,7 +1349,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   }
   __syncwarp();
 
-  PHASE_MARK(4);
+  PHASE_MARK(4);  // crb+M
   PSYNC();
   REGIONS();
   // ---------------- phase 4: velocities, bias forces, actuation, qfrc_smooth ----------------------
@@ -1504,7 +1504,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     }
   }
 
-  PHASE_MARK(5);
+  PHASE_MARK(5);  // vel/rne/act/qfrc_smooth
   PSYNC();
   REGIONS();
   // ---------------- phase 5: collision (static pair table, bounding-sphere filter, primitives) ----
@@ -1630,7 +1630,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
         __syncwarp();
       }
     }
-    PHASE_MARK(17);  // pair-table broadphase
+    PHASE_MARK(17);  // collision: pair-table broadphase
     const float* gsize = MP(geom_size);
     if (m.nstatic > 0) {
       // grid-static candidates: lane = dynamic geom, visiting the cells under its bounding sphere.  Two passes
@@ -1706,7 +1706,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
         ncand += tot;
       }
     }
-    PHASE_MARK(18);  // grid broadphase
+    PHASE_MARK(18);  // collision: grid broadphase
     if (ncand > L.maxpair) { ncand = L.maxpair; overflow = 1; }
     __syncwarp();
     const float* ggap = MP(geom_gap);
@@ -1819,14 +1819,14 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
           }
         }
       }
-      PHASE_MARK(19);  // primitive narrowphase
+      PHASE_MARK(19);  // collision: primitive narrowphase
       if (CVX) {
         if (__any_sync(FULL, hf)) {
           int nh = hfield_lanes(rc, hf, margin, m, gsize, g1, g2, hfa, hfb, (int*)(s + L.gV), lane);
           if (hf) n = nh;
         }
       }
-      PHASE_MARK(20);  // height-field pairs (total of 21-23 + merge)
+      PHASE_MARK(20);  // collision: height-field pairs
       // deterministic compaction in (pair order, contact index) order
       int incl = n;
 #pragma unroll
@@ -1923,7 +1923,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
   }
   __syncwarp();
 
-  PHASE_MARK(6);
+  PHASE_MARK(6);  // collision
   PSYNC();
   REGIONS();
   // ---------------- phase 6: joint-limit rows, body-pair groups ----------------------------------
@@ -2058,7 +2058,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     __syncwarp();
   }
 
-  PHASE_MARK(7);
+  PHASE_MARK(7);  // limits/groups/aref
   PSYNC();
   REGIONS();
   // ---------------- phase 7: unconstrained acceleration -------------------------------------------
@@ -2071,7 +2071,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     #pragma unroll 1
     for (int i = lane; i < nv; i += 32) dd.qacc_smooth.p[(size_t)w * dd.qacc_smooth.stride + i] = qacc_smooth[i];
 
-  PHASE_MARK(8);
+  PHASE_MARK(8);  // chol(M)+qacc_smooth
   PSYNC();
   REGIONS();
   // ---------------- phase 8: Newton solver (primal, exact line search) ----------------------------
@@ -2273,7 +2273,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
       if (niter >= m.iterations) { run = false; break; }
       first = false;
     } while (0);
-    PHASE_MARK(12);
+    PHASE_MARK(12);  // newton: update(J^T f, cost)
     PSYNC();
     REGIONS();
     if (run && !refine && !cg) {
@@ -2349,7 +2349,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
         __syncwarp();
       }
     }
-    PHASE_MARK(13);
+    PHASE_MARK(13);  // newton: H assembly
     PSYNC();
     REGIONS();
     if (run && !cg) {
@@ -2376,7 +2376,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
       }
       __syncwarp();
     }
-    PHASE_MARK(14);
+    PHASE_MARK(14);  // newton: chol+solve
     PSYNC();
     REGIONS();
     if (run) do {
@@ -2453,7 +2453,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
         d1 = fmaxf(wsum(a1) + 2.f * g2, MINVAL);
         nls++;
       };
-      PHASE_MARK(15);
+      PHASE_MARK(15);  // newton: symv+mulJ
       float alpha = 0.f, d0, d1;
       // (slope and curvature at 0 are evaluated rather than derived from grad . search: no measurable time on the GPU,
       // and the worst of 1024 stiff envs of the config-C parity states stays at 1.8e-4 instead of 3.3e-4)
@@ -2477,7 +2477,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
           alpha = nxt;
         }
       }
-      PHASE_MARK(16);
+      PHASE_MARK(16);  // newton: line search
       if (alpha == 0.f) { run = false; break; }
       #pragma unroll 1
       for (int i = lane; i < n; i += 32) { qacc[i] += alpha * search[i]; Ma[i] += alpha * Mv[i]; }
@@ -2520,7 +2520,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     #pragma unroll 1
     for (int i = lane; i < nv; i += 32) asp[i] = qacc_smooth[i];
   }
-  PHASE_MARK(9);
+  PHASE_MARK(9);  // solver total(excl sub)
   PSYNC();
   REGIONS();
   // ---------------- phase 9: contact forces, sensors -----------------------------------------------
@@ -2620,7 +2620,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
     }
   }
 
-  PHASE_MARK(10);
+  PHASE_MARK(10);  // sensors/forces
   PSYNC();
   REGIONS();
   // ---------------- phase 10: integrate (implicitfast / Euler), write state ------------------------
@@ -2710,7 +2710,7 @@ b2_step_kernel(const __grid_constant__ DevModel m, const __grid_constant__ DevDa
       bulk_s2g(gv, qvel, 4u * dd.qvel.stride);
       bulk_commit_wait();
     }
-    PHASE_MARK(11);
+    PHASE_MARK(11);  // integrate+store
     if (lane == 0) {
       dd.ncon.p[(size_t)w * dd.ncon.stride] = ncon;
       dd.nefc.p[(size_t)w * dd.nefc.stride] = nefc;

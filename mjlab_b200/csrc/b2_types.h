@@ -10,12 +10,8 @@
 // instantiations (<0>, <1>) into 128 registers without spills: 16 warps per SM.  The instantiations with the convex
 // routines (<2>, <3>, models with mesh or height-field pairs) spill a few words at 128 and keep 12 warps per SM
 // (up to 168 registers).  DESIGN.md §4.1 has the measurements.
-#ifndef B2_MIN_CTAS
 #define B2_MIN_CTAS (16 / B2_WARPS_PER_CTA)
-#endif
-#ifndef B2_MIN_CTAS_CVX
 #define B2_MIN_CTAS_CVX (12 / B2_WARPS_PER_CTA)
-#endif
 #define B2_MAX_FIELDS 96
 
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };

@@ -1,8 +1,10 @@
 """Aggregate tools/ncu_by_line.py output by kernel phase / helper function.
 
   python tools/ncu_by_phase.py <report.ncu-rep> [kernel-substring]
-Ranges come from the *current* b2_kernel.cuh (out-of-line helpers by their definition lines, kernel phases by
-their PHASE_MARK lines), so the library and source must be the ones the report was captured with."""
+Ranges come from the *current* b2_kernel.cuh, so the library and source must be the ones the report was captured
+with.  A line belongs to the next PHASE_MARK after it (the mark's comment labels the code that ends there), unless an
+out-of-line helper or the kernel itself starts in between; lines of a helper after its last mark count as the helper,
+and lines of the kernel after its last mark as the kernel's tail."""
 import os
 import re
 import subprocess
@@ -10,27 +12,26 @@ import sys
 
 root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 src = open(os.path.join(root, "mjlab_b200", "csrc", "b2_kernel.cuh")).read().splitlines()
-marks = []  # (line, label)
+owner = {}  # source line -> label
+region, pending = "?", []
 for i, ln in enumerate(src, 1):
+  start = None
   m = re.match(r"__device__ __noinline__ \w[\w ]*?(\w+)\(", ln)
   if m:
-    marks.append((i, "fn " + m.group(1)))
-  m = re.match(r"__device__ __forceinline__ \w[\w ]*?(\w+)\(", ln)
+    start = "fn " + m.group(1)
+  if re.match(r"__device__ __forceinline__ \w[\w ]*?(\w+)\(", ln):
+    start = "inline helpers"
+  if ln.startswith("template <int MODE>"):
+    start = "kernel tail (after the last mark)"
+  if start:
+    owner.update((l, region) for l in pending)
+    region, pending = start, []
+  pending.append(i)
+  m = re.match(r"^[ \t]*PHASE_MARK\((\d+)\);[ \t]*//[ \t]*(.*\S)", ln)
   if m:
-    marks.append((i, "inline helpers"))
-  m = re.match(r"\s*PHASE_MARK\((\d+)\);", ln)
-  if m:
-    marks.append((i, "after mark " + m.group(1)))
-  if ln.startswith("template <bool STEP>"):
-    marks.append((i, "kernel prologue / TMA load"))
-names = {"after mark 0": "1 kinematics", "after mark 1": "1b geom/site poses", "after mark 2": "2 com/cinert/cdof",
-         "after mark 3": "3 CRB", "after mark 4": "4 velocities/RNE/actuation", "after mark 5": "5 collision",
-         "after mark 6": "6 limits/groups/aref", "after mark 7": "7 M factor + qacc_smooth",
-         "after mark 8": "8 solver: init + update (J^T f, cost)", "after mark 12": "8 solver: H assembly",
-         "after mark 13": "8 solver: factor/solve calls", "after mark 14": "8 solver: line-search setup",
-         "after mark 15": "8 solver: line search", "after mark 16": "8 solver: move + bookkeeping",
-         "after mark 9": "9 contact forces / sensors", "after mark 10": "10 integrate", "after mark 11": "11 stores"}
-marks.sort()
+    owner.update((l, m.group(1) + " " + m.group(2)) for l in pending)
+    pending = []
+owner.update((l, region) for l in pending)
 out = subprocess.run([sys.executable, os.path.join(root, "tools", "ncu_by_line.py"), sys.argv[1],
                       sys.argv[2] if len(sys.argv) > 2 else "b2_step_kernelILi1", "100000"],
                      capture_output=True, text=True).stdout
@@ -42,13 +43,7 @@ for line in out.splitlines():
       print(line)
     continue
   f, l, sp, ip = m.group(1), int(m.group(2)), float(m.group(3)), float(m.group(4))
-  if f != "b2_kernel.cuh":
-    key = "cuda intrinsics headers (shfl, ...)"
-  else:
-    key = "?"
-    for ml, lab in marks:
-      if ml <= l:
-        key = names.get(lab, lab)
+  key = owner.get(l, "?") if f == "b2_kernel.cuh" else "cuda intrinsics headers (shfl, ...)"
   t = tot.setdefault(key, [0.0, 0.0])
   t[0] += sp
   t[1] += ip

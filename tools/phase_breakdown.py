@@ -1,19 +1,18 @@
-"""Per-phase cycle breakdown of the step kernel (needs the -DB2_PHASE_TIMING variant:
-B2SIM_LIB=mjlab_b200/csrc/variants/libb2sim_timing.so python tools/phase_breakdown.py)."""
-import ctypes, sys
+"""Per-phase cycle breakdown of the step kernel on one of bench.py's workloads (needs the -DB2_PHASE_TIMING variant):
+  B2SIM_LIB=mjlab_b200/csrc/variants/libb2sim_timing.so python tools/phase_breakdown.py [envs] [preroll] [opt=val ...]
+B2_WORKLOAD (B, C, E or F, default B) picks the workload.
+Each row is the code that ends at one PHASE_MARK of b2_kernel.cuh, labelled by the comment on that mark."""
+import ctypes, os, re, sys
 from pathlib import Path
-sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+ROOT = Path(__file__).resolve().parents[1]
+sys.path.insert(0, str(ROOT))
 import torch
-from mjlab_b200.envs import VelocityEnvCfg, VelocityFlatEnv
+import bench
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
-import os
-_wl = os.environ.get("B2_WORKLOAD", "B")  # B: G1 flat, E: Go1 rough boxes, F: Go1 rough boxes + height fields
-_kw = dict(B={}, E=dict(robot="go1", terrain="rough"), F=dict(robot="go1", terrain="rough_hf"))[_wl]
-env = VelocityFlatEnv(VelocityEnvCfg(num_envs=n, **_kw), device="cuda:0")
-_nu = env.nu if hasattr(env, "nu") else (29 if _wl == "B" else 12)
+env = bench.make_env(os.environ.get("B2_WORKLOAD", "B"), n, 42, "cuda:0")
 g = torch.Generator(device="cuda:0"); g.manual_seed(0)
 for _ in range(int(sys.argv[2]) if len(sys.argv) > 2 else 100):
-  env.step(torch.rand((n, _nu), generator=g, device="cuda:0") * 2 - 1)
+  env.step(torch.rand((n, env.nu), generator=g, device="cuda:0") * 2 - 1)
 sim = env.sim
 for kv in sys.argv[3:]:
   k, v = kv.split("=")
@@ -24,14 +23,11 @@ K = 20
 for _ in range(K): sim.step()
 torch.cuda.synchronize()
 assert sim._lib.b2_phase_cycles(buf) == 0, "library built without -DB2_PHASE_TIMING"
-names = ["load(TMA)", "kinematics", "geom/site poses", "com/cinert/cdof", "crb+M", "vel/rne/act/qfrc_smooth",
-         "collision", "limits/groups/aref", "chol(M)+qacc_smooth", "solver total(excl sub)", "sensors/forces",
-         "integrate+store", "  newton: update(J^T f, cost)", "  newton: H assembly", "  newton: chol+solve",
-         "  newton: symv+mulJ", "  newton: line search", "  collision: pair-table broadphase",
-         "  collision: grid broadphase", "  collision: primitive narrowphase", "  collision: height-field pairs",
-         "    (hfield: footprints)", "    (hfield: cull)", "    (hfield: prisms + merge)"]
+src = (ROOT / "mjlab_b200" / "csrc" / "b2_kernel.cuh").read_text()
+labels = {int(k): lab for k, lab in re.findall(r"^[ \t]*PHASE_MARK\((\d+)\);[ \t]*//[ \t]*(.*\S)", src, re.M)}
+# marks 21-23 run inside the height-field routine and split the time of mark 20, so the total is marks 0-20
 tot = sum(buf[i] for i in range(21))
 st = sim.stats()
 print(f"mean newton iters {st.niter_mean:.2f}, mean ncon {st.ncon_mean:.1f}; cycles per env-step (warp-serial): {tot / (K * n):.0f}")
-for i, nm in enumerate(names):
-  print(f"{nm:34s} {buf[i] / (K * n):10.0f} cyc/env  {100.0 * buf[i] / tot:5.1f}%")
+for i in sorted(labels):
+  print(f"{i:2d} {labels[i]:34s} {buf[i] / (K * n):10.0f} cyc/env  {100.0 * buf[i] / tot:5.1f}%")

@@ -1,21 +1,18 @@
-"""Profiling driver: bring 4096 G1 envs into the steady-state workload distribution (random
-actions with resets), then run a few physics steps for ncu / timing experiments."""
-import sys, time
+"""Profiling driver: bring n environments of one of bench.py's workloads (B2_WORKLOAD, default B) into the
+steady-state workload distribution (random actions with resets), then run a few physics steps for ncu / timing
+experiments."""
+import os, sys
 from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import torch
-from mjlab_b200.envs import VelocityEnvCfg, VelocityFlatEnv
+import bench
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 mode = sys.argv[2] if len(sys.argv) > 2 else "time"
-import os
-_wl = os.environ.get("B2_WORKLOAD", "B")  # B: G1 flat, E: Go1 rough boxes, F: Go1 rough boxes + height fields
-_kw = dict(B={}, E=dict(robot="go1", terrain="rough"), F=dict(robot="go1", terrain="rough_hf"))[_wl]
-env = VelocityFlatEnv(VelocityEnvCfg(num_envs=n, **_kw), device="cuda:0")
-_nu = 29 if _wl == "B" else 12
+env = bench.make_env(os.environ.get("B2_WORKLOAD", "B"), n, 42, "cuda:0")
 g = torch.Generator(device="cuda:0"); g.manual_seed(0)
 for _ in range(int(sys.argv[3]) if len(sys.argv) > 3 else 60):
-  env.step(torch.rand((n, _nu), generator=g, device="cuda:0") * 2 - 1)
+  env.step(torch.rand((n, env.nu), generator=g, device="cuda:0") * 2 - 1)
 torch.cuda.synchronize()
 sim = env.sim
 def timeit(label, k=20):
@@ -49,5 +46,5 @@ if mode == "time":
   sim.data.qpos[:, 2] += 5.0  # lift everyone: no contacts
   timeit("airborne (no contacts)")
 else:
-  for _ in range(6): sim.step_n(1) if hasattr(sim, "step_n") else sim.step()
+  for _ in range(6): sim.step_n(1)
   torch.cuda.synchronize()
