@@ -113,6 +113,7 @@ int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_ho
  * ManagerBasedRlEnv.step (manager_based_rl_env.py:106-147) does before and after the decimation loop for
  * tasks/velocity/velocity_env_cfg.py, as two launches. All pointers are device pointers. */
 #define B2_VELENV_NU(nu) (16 + 9 + 2 * (nu))
+#define B2_VELENV_NTERM 14 /* reward terms with an episode sum (B2VelEnvArgs.rewards) */
 typedef struct B2VelEnvArgs {
   const float* action;            /* [n][nu] */
   const float* U;                 /* [n][B2_VELENV_NU(nu)] uniforms in [0,1): 0-1 reset xy, 2 yaw, 3-5 command, 6 heading
@@ -151,6 +152,37 @@ typedef struct B2VelEnvArgs {
   float* terrain_level_mean;      /* [1] out: mean of terrain_levels after the update (the curriculum's log value) */
   float move_up_dist, episode_length_s;
   int32_t rows, cols, curriculum;
+  /* opt-in reward terms of the reference's velocity task (tasks/velocity/mdp/rewards.py:52-190) and shared penalties
+   * (envs/mdp/rewards.py:22-127), with per-term episode sums (managers/reward_manager.py:61-89); rewards = 0 leaves
+   * every field below unread.  Terms, in the order of the episode-sum columns (B2_VELENV_NTERM):
+   *   0-4 the fixed terms: track_lin_vel_exp, track_ang_vel_exp, pose, dof_pos_limits, action_rate_l2 (weights 1, 1,
+   *       1, -1, -0.1, not configurable);
+   *   5 air_time, 6 feet_slide, 7 foot_clearance, 8 is_alive, 9 is_terminated, 10 joint_torques_l2, 11 joint_acc_l2,
+   *   12 electrical_power_cost, 13 flat_orientation_l2.
+   * A term at weight 0 is not evaluated and the air-time state does not advance.  reward = (fixed terms + sum of
+   * w_i r_i) step_dt.  A foot is in contact when sensordata[adr] > 0; a geom's linear velocity is
+   * cvel[3:6] - cvel[0:3] x (subtree_com[root_body] - geom_xpos).  Per-foot state of a done env is zeroed after its
+   * reward.  episode_sums[w][i] += w_i r_i step_dt for all 14 terms; a done env's row is copied to finished_sums and
+   * zeroed.  A null episode_sums skips both. */
+  float weight[B2_VELENV_NTERM - 5]; /* of terms 5-13 */
+  float air_threshold_min, air_threshold_max, air_command_threshold, air_command_scale_width;
+  float clearance_target_height, clearance_std, clearance_tanh_mult;
+  int32_t air_continuous;         /* reward_mode: 0 "on_landing", 1 "continuous" */
+  int32_t air_hard_scale;         /* command_scale_type: 0 "smooth", 1 "hard" */
+  int32_t n_air, n_slide, n_clear; /* feet of each term, <= 32 */
+  int32_t root_body;              /* body whose subtree_com the geom velocities are taken about */
+  const int32_t* air_sensor_adr;  /* [n_air] sensordata address of each foot's contact sensor */
+  const int32_t* slide_sensor_adr; /* [n_slide] */
+  const int32_t* slide_geom;      /* [n_slide] */
+  const int32_t* slide_body;      /* [n_slide] body of each geom */
+  const int32_t* clear_geom;      /* [n_clear] */
+  const int32_t* clear_body;      /* [n_clear] */
+  float* air_time;                /* [n][n_air] in/out: current air time */
+  float* contact_time;            /* [n][n_air] in/out: current contact time */
+  float* last_air_time;           /* [n][n_air] in/out: air time of the last landing */
+  float* episode_sums;            /* [n][B2_VELENV_NTERM] in/out, or null */
+  float* finished_sums;           /* [n][B2_VELENV_NTERM] out: the sums of the episode a done env just ended */
+  int32_t rewards;
 } B2VelEnvArgs;
 int b2_velenv_pre(b2_sim* sim, const float* action, const float* default_joint_pos,
                   const float* action_scale, void* cuda_stream);

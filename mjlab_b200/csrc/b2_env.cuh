@@ -2,7 +2,8 @@
 // 1-3): the caller-side work of ManagerBasedRlEnv.step (reference src/mjlab/envs/manager_based_rl_env.py:106-147
 // with the terms of tasks/velocity/velocity_env_cfg.py) as two kernels instead of ~90 tiny torch launches:
 //   pre  : ctrl = default_joint_pos + action_scale * action                     (joint_actions.py:85-103)
-//   post : episode counter, terminations (bad_orientation, time_out), rewards, the terrain-level curriculum of
+//   post : episode counter, terminations (bad_orientation, time_out), rewards (the five fixed terms, the opt-in terms
+//          of B2VelEnvArgs.rewards and their episode sums), the terrain-level curriculum of
 //          the reset envs (opt-in, curriculums.py:18-52), masked reset (events.py:43-124), interval push
 //          (events.py:127-143), command resample, observations.
 // The torch implementation in mjlab_b200/envs/velocity_env.py is the reference; both consume the same
@@ -43,9 +44,11 @@ __device__ __forceinline__ float b2e_wsum(float v) {
 // contraction), but a terrain level must move exactly as on the torch path
 #ifdef B2_HOST_EMULATION
 __device__ __forceinline__ float b2e_mul_rn(float a, float b) { return a * b; }
+__device__ __forceinline__ float b2e_add_rn(float a, float b) { return a + b; }
 __device__ __forceinline__ float b2e_norm2_rn(float x, float y) { return sqrtf(x * x + y * y); }
 #else
 __device__ __forceinline__ float b2e_mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float b2e_add_rn(float a, float b) { return __fadd_rn(a, b); }
 __device__ __forceinline__ float b2e_norm2_rn(float x, float y) {
   return __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
 }
@@ -65,6 +68,43 @@ __device__ __forceinline__ void b2e_terrain_level(const B2VelEnvArgs& A, int w, 
   A.terrain_levels[w] = level;
   const float* src = A.terrain_origins + 3 * ((size_t)level * A.cols + A.terrain_types[w]);
   org[0] = src[0]; org[1] = src[1]; org[2] = src[2];
+}
+
+// World-frame linear velocity (x, y) and height of geom g on body b (EntityData.geom_vel_w, entity/data.py:20-31,
+// 282-288): cvel[3:6] - cvel[0:3] x (subtree_com[root] - geom_xpos).
+__device__ __forceinline__ void b2e_geom_vel(const DevData& dd, int w, int g, int b, int root, float& vx, float& vy,
+                                             float& z) {
+  const float* p = dd.geom_xpos.p + (size_t)w * dd.geom_xpos.stride + 3 * g;
+  const float* s = dd.subtree_com.p + (size_t)w * dd.subtree_com.stride + 3 * root;
+  const float* c = dd.cvel.p + (size_t)w * dd.cvel.stride + 6 * b;
+  const float o0 = s[0] - p[0], o1 = s[1] - p[1], o2 = s[2] - p[2];
+  vx = c[3] - (c[1] * o2 - c[2] * o1);
+  vy = c[4] - (c[2] * o0 - c[0] * o2);
+  z = p[2];
+}
+
+// feet_air_time (tasks/velocity/mdp/rewards.py:52-146) on one lane per foot: advances the foot's state (zeroed when
+// the env is done, as reset(env_ids) does) and returns the warp's reward before the command scale.
+__device__ __forceinline__ float b2e_air_time(const B2VelEnvArgs& A, const float* sd, int w, int lane, bool done) {
+  float r = 0.f;
+  if (lane < A.n_air) {
+    const size_t k = (size_t)w * A.n_air + lane;
+    const bool contact = sd[A.air_sensor_adr[lane]] > 0.f;
+    float air = A.air_time[k], ct = A.contact_time[k], last = A.last_air_time[k];
+    const bool first = air > 0.f && contact;  // landing: from the air time before this step's update
+    if (first) last = air;
+    air = contact ? 0.f : b2e_add_rn(air, A.step_dt);
+    ct = contact ? b2e_add_rn(ct, A.step_dt) : 0.f;
+    if (A.air_continuous)
+      r = !contact && air > A.air_threshold_min && air <= A.air_threshold_max ? 1.f : 0.f;
+    else if (first)
+      r = fminf(fmaxf(last - A.air_threshold_min, 0.f), A.air_threshold_max - A.air_threshold_min);
+    A.air_time[k] = done ? 0.f : air;
+    A.contact_time[k] = done ? 0.f : ct;
+    A.last_air_time[k] = done ? 0.f : last;
+  }
+  r = b2e_wsum(r);
+  return A.air_continuous ? r : r / A.step_dt;
 }
 
 // One warp per environment (a thread per environment left 4096 threads = 128 warps on 132 SMs walking ~400
@@ -107,15 +147,80 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     rate += da * da;
   }
   pose = b2e_wsum(pose); lim = b2e_wsum(lim); rate = b2e_wsum(rate);
+  bool done = term || trunc;
+  // opt-in terms (B2VelEnvArgs.rewards): r[i] is term 5 + i unweighted, evaluated only at a non-zero weight
+  float r[B2_VELENV_NTERM - 5] = {}, extra = 0.f;
+  bool any = false;
+  if (A.rewards) {
+    const float* W = A.weight;
+    const float* sd = dd.sensordata.p + (size_t)w * dd.sensordata.stride;
+    if (W[0] != 0.f) {  // air_time, scaled by the command (smooth or hard)
+      const float cn = b2e_norm2_rn(c0, c1);
+      const float s = A.air_hard_scale ? (cn > A.air_command_threshold ? 1.f : 0.f)
+                                       : 0.5f * (1.f + tanhf((cn - A.air_command_threshold) / A.air_command_scale_width));
+      r[0] = b2e_air_time(A, sd, w, lane, done) * s;
+    }
+    if (W[1] != 0.f) {  // feet_slide
+      float v = 0.f;
+      if (lane < A.n_slide && sd[A.slide_sensor_adr[lane]] > 0.f) {
+        float vx, vy, z;
+        b2e_geom_vel(dd, w, A.slide_geom[lane], A.slide_body[lane], A.root_body, vx, vy, z);
+        v = sqrtf(vx * vx + vy * vy);
+      }
+      r[1] = b2e_wsum(v);
+    }
+    if (W[2] != 0.f) {  // foot_clearance_reward
+      float v = 0.f;
+      if (lane < A.n_clear) {
+        float vx, vy, z;
+        b2e_geom_vel(dd, w, A.clear_geom[lane], A.clear_body[lane], A.root_body, vx, vy, z);
+        const float e = z - A.clearance_target_height;
+        v = e * e * tanhf(A.clearance_tanh_mult * sqrtf(vx * vx + vy * vy));
+      }
+      r[2] = expf(-b2e_wsum(v) / A.clearance_std);
+    }
+    r[3] = term ? 0.f : 1.f;  // is_alive
+    r[4] = term ? 1.f : 0.f;  // is_terminated
+    if (W[5] != 0.f || W[6] != 0.f || W[7] != 0.f) {  // joint_torques_l2, joint_acc_l2, electrical_power_cost
+      const float* af = dd.actuator_force.p + (size_t)w * dd.actuator_force.stride;
+      const float* qa = dd.qacc.p + (size_t)w * dd.qacc.stride;
+      float tau = 0.f, acc = 0.f, pw = 0.f;
+      for (int a = lane; a < nu; a += 32) {
+        const float f = af[a], j = qa[6 + a];
+        tau += f * f;
+        acc += j * j;
+        pw += fmaxf(f * qvel[6 + a], 0.f);
+      }
+      r[5] = b2e_wsum(tau); r[6] = b2e_wsum(acc); r[7] = b2e_wsum(pw);
+    }
+    r[8] = gb[0] * gb[0] + gb[1] * gb[1];  // flat_orientation_l2
+#pragma unroll
+    for (int i = 0; i < B2_VELENV_NTERM - 5; i++) {
+      r[i] = W[i] != 0.f ? r[i] * W[i] : 0.f;  // (a term at weight 0 adds nothing, not 0 * its value)
+      any = any || W[i] != 0.f;
+      extra += r[i];
+    }
+  }
   __syncwarp();  // every lane holds the pre-reset state it needs; writes may start
   float r_pose = expf(-(pose / (float)nu) / 0.09f);
-  const float reward = (r_lin + r_ang + r_pose - lim - 0.1f * rate) * A.step_dt;
-  bool done = term || trunc;
+  const float fixed = r_lin + r_ang + r_pose - lim - 0.1f * rate;
+  const float reward = any ? (fixed + extra) * A.step_dt : fixed * A.step_dt;
   if (lane == 0) {
     A.reward[w] = reward;
     A.terminated[w] = term; A.truncated[w] = trunc; A.done[w] = done;
     A.log_row[3 * (size_t)w] = reward; A.log_row[3 * (size_t)w + 1] = term ? 1.f : 0.f;
     A.log_row[3 * (size_t)w + 2] = trunc ? 1.f : 0.f;
+  }
+  // episode sums (RewardManager.compute / reset): column k on lane k
+  if (A.rewards && A.episode_sums && lane < B2_VELENV_NTERM) {
+    float v = lane == 0 ? r_lin : lane == 1 ? r_ang : lane == 2 ? r_pose : lane == 3 ? -lim : lane == 4 ? -0.1f * rate : 0.f;
+#pragma unroll
+    for (int i = 0; i < B2_VELENV_NTERM - 5; i++)
+      if (lane == 5 + i) v = r[i];
+    const size_t k = (size_t)w * B2_VELENV_NTERM + lane;
+    const float s = A.episode_sums[k] + v * A.step_dt;
+    if (done) A.finished_sums[k] = s;
+    A.episode_sums[k] = done ? 0.f : s;
   }
   // masked reset (reset_root_state_uniform + reset_joints_by_scale), command resample
   if (done) {
@@ -186,10 +291,12 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   if (lane < 3) {
     const int k = lane;
     const float av = qvel[3 + k];
-    cr[k] = lb[k]; cr[3 + k] = av; cr[6 + k] = gb[k];
-    o[k] = lb[k] + (Z[k] * 2.f - 1.f) * 0.1f;
+    // (selects, not lb[k]: an array indexed by the lane would be placed in local memory)
+    const float lk = k == 0 ? lb[0] : (k == 1 ? lb[1] : lb[2]), gk = k == 0 ? gb[0] : (k == 1 ? gb[1] : gb[2]);
+    cr[k] = lk; cr[3 + k] = av; cr[6 + k] = gk;
+    o[k] = lk + (Z[k] * 2.f - 1.f) * 0.1f;
     o[3 + k] = av + (Z[3 + k] * 2.f - 1.f) * 0.2f;
-    o[6 + k] = gb[k] + (Z[6 + k] * 2.f - 1.f) * 0.05f;
+    o[6 + k] = gk + (Z[6 + k] * 2.f - 1.f) * 0.05f;
     const float ck = k == 0 ? c0 : (k == 1 ? c1 : c2);
     o[9 + 3 * nu + k] = ck; cr[9 + 3 * nu + k] = ck;
   }

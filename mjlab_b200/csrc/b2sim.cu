@@ -1096,6 +1096,17 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
        !args->terrain_level_mean || args->rows < 1 || args->cols < 1))
     return fail("b2_velenv_post: the terrain curriculum needs env_origins, terrain_origins, terrain_levels, "
                 "terrain_types, terrain_level_mean and rows, cols >= 1");
+  if (args->rewards) {
+    const B2VelEnvArgs& a = *args;
+    const float* W = a.weight;
+    const bool feet_ok = a.n_air >= 0 && a.n_air <= 32 && a.n_slide >= 0 && a.n_slide <= 32 && a.n_clear >= 0 &&
+                         a.n_clear <= 32 && a.root_body >= 0 && a.root_body < s->hm.nbody;
+    if (!feet_ok || (W[0] != 0.f && (!a.air_sensor_adr || !a.air_time || !a.contact_time || !a.last_air_time)) ||
+        (W[1] != 0.f && (!a.slide_sensor_adr || !a.slide_geom || !a.slide_body)) ||
+        (W[2] != 0.f && (!a.clear_geom || !a.clear_body)) || (a.episode_sums && !a.finished_sums))
+      return fail("b2_velenv_post: the reward terms need at most 32 feet each, a valid root_body, the arrays of "
+                  "every term with a non-zero weight, and finished_sums beside episode_sums");
+  }
   DeviceGuard guard(s->device);
   b2_velenv_post_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(  // one warp per environment
       s->hd, s->hm.nq, s->hm.nv, s->hm.nu, *args);

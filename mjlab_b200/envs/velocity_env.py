@@ -22,6 +22,45 @@ from mjlab_b200.asset_zoo import g1, go1, load_compiled
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
 
 
+REWARD_TERMS = ("track_lin_vel_exp", "track_ang_vel_exp", "pose", "dof_pos_limits", "action_rate_l2",  # fixed
+                "air_time", "feet_slide", "foot_clearance", "is_alive", "is_terminated", "joint_torques_l2",
+                "joint_acc_l2", "electrical_power_cost", "flat_orientation_l2")  # opt-in (VelocityRewardsCfg)
+NFIXED = 5
+
+
+@dataclass
+class VelocityRewardsCfg:
+  """Reward terms the reference's velocity task offers beside the five fixed ones (tasks/velocity/mdp/rewards.py:52-190,
+  envs/mdp/rewards.py:22-127), each off at weight 0: a term at weight 0 is not evaluated and its state does not
+  advance (reward_manager.py:82-84).  Sensor and geom names are the robot's own (without the ``robot/`` prefix)."""
+
+  air_time: float = 0.0
+  feet_slide: float = 0.0
+  foot_clearance: float = 0.0
+  is_alive: float = 0.0
+  is_terminated: float = 0.0
+  joint_torques_l2: float = 0.0
+  joint_acc_l2: float = 0.0
+  electrical_power_cost: float = 0.0
+  flat_orientation_l2: float = 0.0
+  # feet_air_time (velocity_env_cfg.py:201-214); sensor_names None: the model's *_foot_ground_contact sensors
+  air_time_sensor_names: tuple | None = None
+  threshold_min: float = 0.05
+  threshold_max: float = 0.15
+  command_threshold: float = 0.05
+  reward_mode: str = "on_landing"          # "on_landing" | "continuous"
+  command_scale_type: str = "smooth"       # "smooth" | "hard"
+  command_scale_width: float = 0.2
+  # feet_slide: one geom per contact sensor
+  feet_slide_sensor_names: tuple = ()
+  feet_slide_geom_names: tuple = ()
+  # foot_clearance_reward: no defaults in the reference, required at a non-zero weight
+  target_height: float | None = None
+  std: float | None = None
+  tanh_mult: float | None = None
+  foot_clearance_geom_names: tuple = ()
+
+
 @dataclass
 class VelocityEnvCfg:
   robot: str = "g1"
@@ -46,6 +85,7 @@ class VelocityEnvCfg:
       mujoco=MujocoCfg(timestep=0.005, iterations=10, ls_iterations=20),
     )
   )
+  rewards: VelocityRewardsCfg = field(default_factory=VelocityRewardsCfg)  # opt-in terms beside the fixed five
 
 
 def _resolve(pattern_map: dict, names: list[str], default: float) -> list[float]:
@@ -141,6 +181,7 @@ class VelocityFlatEnv:
     self._done_buf = torch.zeros(n, dtype=torch.bool, device=dev)  # fixed address (graph capture / native)
     lo_t, hi_t = cfg.push_interval_s
     self.push_time_left.copy_(self._rand(n) * (hi_t - lo_t) + lo_t)
+    self._init_rewards()
     if self.native_mdp:
       self._init_native()
     self._reset_all(curriculum=False)  # no episode has ended yet: the initial levels stand
@@ -154,6 +195,70 @@ class VelocityFlatEnv:
     3-5 command, 6 heading target, 7 standing draw, 8 command timer, 9-10 push, 11 push timer, 12 terrain level
     redraw, 16.. obs noise."""
     return self._rand(self.num_envs, 16 + 9 + 2 * self.nu)
+
+  def _init_rewards(self) -> None:
+    """Resolve VelocityRewardsCfg against the model and allocate the air-time state and the episode sums."""
+    rc, m, n = self.cfg.rewards, self.model, self.num_envs
+    if rc.reward_mode not in ("on_landing", "continuous"):
+      raise ValueError(f"reward_mode must be 'on_landing' or 'continuous', not {rc.reward_mode!r}")
+    if rc.command_scale_type not in ("smooth", "hard"):
+      raise ValueError(f"command_scale_type must be 'smooth' or 'hard', not {rc.command_scale_type!r}")
+    self.reward_weights = [float(getattr(rc, t)) for t in REWARD_TERMS[NFIXED:]]
+    sensors, geoms, intprm = m.names["sensor"], m.names["geom"], np.asarray(m.arrays["sensor_intprm"]).reshape(-1, 3)
+
+    def lookup(kind, names, table):
+      if len(names) > 32:
+        raise ValueError(f"at most 32 feet per reward term, got {len(names)} {kind}s")
+      ids = []
+      for s in names:
+        if f"robot/{s}" not in table:
+          raise ValueError(f"unknown {kind} '{s}'")
+        ids.append(table.index(f"robot/{s}"))
+      return ids
+
+    def contact_adr(names):
+      ids = lookup("sensor", names, sensors)
+      for s, i in zip(names, ids):
+        if not intprm[i, 0] & 1:  # the data fields are packed found, force, ... (compiler/spec.py CONTACT_DATA)
+          raise ValueError(f"sensor '{s}': its first data field is not 'found'")
+      return [int(m.arrays["sensor_adr"][i]) for i in ids]
+
+    air_names = rc.air_time_sensor_names
+    if air_names is None:
+      air_names = [s.split("/", 1)[1] for s in sensors if s.startswith("robot/") and s.endswith("_foot_ground_contact")]
+    if len(rc.feet_slide_sensor_names) != len(rc.feet_slide_geom_names):
+      raise ValueError(f"feet_slide needs one geom per sensor: {len(rc.feet_slide_sensor_names)} sensors, "
+                       f"{len(rc.feet_slide_geom_names)} geoms")
+    w_air, w_slide, w_clear = self.reward_weights[:3]
+    if w_clear != 0.0 and None in (rc.target_height, rc.std, rc.tanh_mult):
+      raise ValueError("foot_clearance needs target_height, std and tanh_mult")
+    for w_, k, names in ((w_air, "air_time", air_names), (w_slide, "feet_slide", rc.feet_slide_sensor_names),
+                         (w_clear, "foot_clearance", rc.foot_clearance_geom_names)):
+      if w_ != 0.0 and not names:
+        raise ValueError(f"{k} has a non-zero weight and no feet")
+    i32 = dict(dtype=torch.int32, device=self.device)
+    body = np.asarray(m.arrays["geom_bodyid"])
+    self._air_adr = torch.tensor(contact_adr(air_names), **i32)
+    self._slide_adr = torch.tensor(contact_adr(rc.feet_slide_sensor_names), **i32)
+    self._slide_geom = torch.tensor(lookup("geom", rc.feet_slide_geom_names, geoms), **i32)
+    self._clear_geom = torch.tensor(lookup("geom", rc.foot_clearance_geom_names, geoms), **i32)
+    self._slide_body, self._clear_body = (torch.tensor(body[g.cpu().numpy()], **i32)
+                                          for g in (self._slide_geom, self._clear_geom))
+    self._root_body = int(m.arrays["body_rootid"][m.arrays["jnt_bodyid"][0]])  # the floating base's tree
+    f32 = dict(dtype=torch.float32, device=self.device)
+    nf = len(air_names)
+    self.air_time, self.contact_time, self.last_air_time = (torch.zeros(n, nf, **f32) for _ in range(3))
+    self.episode_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
+    self.finished_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
+
+  def reward_log(self) -> dict:
+    """``Episode_Reward/<term>`` of RewardManager.reset (managers/reward_manager.py:61-75) for the envs whose episode
+    ended in the last step: the mean of their episode sums over episode_length_s (NaN when none ended), for the fixed
+    terms and the enabled ones.  Device tensors, no host synchronisation."""
+    done = self._done_buf.unsqueeze(1)
+    mean = torch.where(done, self.finished_sums, 0.0).sum(0) / done.sum() / self.cfg.episode_length_s
+    return {f"Episode_Reward/{t}": mean[i] for i, t in enumerate(REWARD_TERMS)
+            if i < NFIXED or self.reward_weights[i - NFIXED] != 0.0}
 
   def _init_native(self) -> None:
     from mjlab_b200.sim import native
@@ -192,6 +297,22 @@ class VelocityFlatEnv:
       a.move_up_dist, a.episode_length_s = self.move_up_dist, self.cfg.episode_length_s
       a.rows, a.cols = self.terrain_origins.shape[:2]
       a.curriculum = 1
+    rc = self.cfg.rewards
+    for name, t in (("air_sensor_adr", self._air_adr), ("slide_sensor_adr", self._slide_adr),
+                    ("slide_geom", self._slide_geom), ("slide_body", self._slide_body), ("clear_geom", self._clear_geom),
+                    ("clear_body", self._clear_body), ("air_time", self.air_time), ("contact_time", self.contact_time),
+                    ("last_air_time", self.last_air_time), ("episode_sums", self.episode_sums),
+                    ("finished_sums", self.finished_sums)):
+      assert t.is_contiguous()
+      setattr(a, name, t.data_ptr())
+    a.weight[:] = self.reward_weights
+    a.air_threshold_min, a.air_threshold_max = rc.threshold_min, rc.threshold_max
+    a.air_command_threshold, a.air_command_scale_width = rc.command_threshold, rc.command_scale_width
+    a.clearance_target_height, a.clearance_std, a.clearance_tanh_mult = (
+      0.0 if v is None else v for v in (rc.target_height, rc.std, rc.tanh_mult))
+    a.air_continuous, a.air_hard_scale = rc.reward_mode == "continuous", rc.command_scale_type == "hard"
+    a.n_air, a.n_slide, a.n_clear = len(self._air_adr), len(self._slide_adr), len(self._clear_geom)
+    a.root_body, a.rewards = self._root_body, 1
     self._native_args = a
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
@@ -231,6 +352,56 @@ class VelocityFlatEnv:
     new = self.terrain_origins[self.terrain_levels.long(), self.terrain_types.long()]
     self.env_origins.copy_(torch.where(mask.unsqueeze(1), new, o))
     self.terrain_level_mean.copy_(self.terrain_levels.float().mean())
+
+  def _geom_vel(self, geoms: torch.Tensor, bodies: torch.Tensor):
+    """Height and world-frame linear velocity of geoms (EntityData.geom_vel_w, entity/data.py:20-31, 282-288)."""
+    d = self.sim.data
+    pos = d.geom_xpos[:, geoms.long()]
+    cvel = d.cvel[:, bodies.long()]
+    com = d.subtree_com[:, self._root_body].unsqueeze(1)
+    return pos[..., 2], cvel[..., 3:6] - torch.cross(cvel[..., 0:3], com - pos, dim=-1)
+
+  def _opt_in_rewards(self, terminated: torch.Tensor, done: torch.Tensor, grav_b: torch.Tensor) -> torch.Tensor:
+    """The VelocityRewardsCfg terms from the pre-reset state, weighted ([n, 9]; zero for a term at weight 0, which is
+    not evaluated).  Advances the air-time state, and zeroes it for the done envs (feet_air_time.reset)."""
+    rc, d, W = self.cfg.rewards, self.sim.data, self.reward_weights
+    out = torch.zeros(self.num_envs, len(W), device=self.device)
+    if W[0] != 0.0:  # feet_air_time (tasks/velocity/mdp/rewards.py:84-146)
+      contact = d.sensordata[:, self._air_adr.long()] > 0
+      first = (self.air_time > 0) & contact
+      last = torch.where(first, self.air_time, self.last_air_time)
+      air = torch.where(contact, 0.0, self.air_time + self.step_dt)
+      ct = torch.where(contact, self.contact_time + self.step_dt, 0.0)
+      if rc.reward_mode == "continuous":
+        r = (~contact & (air > rc.threshold_min) & (air <= rc.threshold_max)).float().sum(1)
+      else:  # the span as the kernel forms it: one fp32 subtraction
+        span = float(np.float32(rc.threshold_max) - np.float32(rc.threshold_min))
+        r = ((last - rc.threshold_min).clamp(min=0.0).clamp(max=span) * first).sum(1) / self.step_dt
+      c = self.command
+      cn = torch.sqrt(c[:, 0] * c[:, 0] + c[:, 1] * c[:, 1])
+      if rc.command_scale_type == "smooth":
+        r = r * (0.5 * (1.0 + torch.tanh((cn - rc.command_threshold) / rc.command_scale_width)))
+      else:
+        r = r * (cn > rc.command_threshold)
+      out[:, 0] = r
+      keep = ~done.unsqueeze(1)
+      for t, v in ((self.air_time, air), (self.contact_time, ct), (self.last_air_time, last)):
+        t.copy_(torch.where(keep, v, 0.0))
+    if W[1] != 0.0:  # feet_slide (:174-187)
+      _, v = self._geom_vel(self._slide_geom, self._slide_body)
+      out[:, 1] = (v[..., :2].norm(dim=-1) * (d.sensordata[:, self._slide_adr.long()] > 0)).sum(1)
+    if W[2] != 0.0:  # foot_clearance_reward (:156-171)
+      z, v = self._geom_vel(self._clear_geom, self._clear_body)
+      err = (z - rc.target_height) ** 2 * torch.tanh(rc.tanh_mult * v[..., :2].norm(dim=-1))
+      out[:, 2] = torch.exp(-err.sum(1) / rc.std)
+    nu = self.nu
+    tau, qd = d.actuator_force[:, :nu], d.qvel[:, 6:]
+    for i, f in ((3, lambda: (~terminated).float()), (4, lambda: terminated.float()),  # envs/mdp/rewards.py:22-127
+                 (5, lambda: (tau ** 2).sum(1)), (6, lambda: (d.qacc[:, 6:] ** 2).sum(1)),
+                 (7, lambda: (tau * qd).clamp(min=0.0).sum(1)), (8, lambda: (grav_b[:, :2] ** 2).sum(1))):
+      if W[i] != 0.0:
+        out[:, i] = f()
+    return out * torch.tensor(W, device=self.device)
 
   def _update_command(self, done: torch.Tensor, U: torch.Tensor) -> None:
     """CommandTerm.compute + UniformVelocityCommand (tasks/velocity/mdp/velocity_command.py:64-110): resample on
@@ -272,6 +443,9 @@ class VelocityFlatEnv:
 
   def _reset_all(self, curriculum: bool):
     all_ = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
+    self.finished_sums.copy_(self.episode_sums)  # RewardManager.reset of every env
+    for t in (self.episode_sums, self.air_time, self.contact_time, self.last_air_time):
+      t.zero_()
     U = self._draw()
     if curriculum:
       self._terrain_curriculum(all_, U)
@@ -364,9 +538,17 @@ class VelocityFlatEnv:
     r_pose = torch.exp(-((jp - self.default_joint_pos) ** 2).mean(1) / 0.09)
     r_lim = -((self.soft_lo - jp).clamp(min=0) + (jp - self.soft_hi).clamp(min=0)).sum(1)
     r_rate = -0.1 * ((action - self.last_action) ** 2).sum(1)
-    reward = (r_lin + r_ang + r_pose + r_lim + r_rate) * self.step_dt
-    self.last_action.copy_(action)
     done = terminated | truncated
+    extra = self._opt_in_rewards(terminated, done, grav_b)  # [n, 9] weighted values of the opt-in terms
+    if any(w != 0.0 for w in self.reward_weights):
+      reward = (r_lin + r_ang + r_pose + r_lim + r_rate + extra.sum(1)) * self.step_dt
+    else:
+      reward = (r_lin + r_ang + r_pose + r_lim + r_rate) * self.step_dt
+    # episode sums (RewardManager.compute / reset): a done env's row ends its episode
+    sums = self.episode_sums + torch.cat([torch.stack([r_lin, r_ang, r_pose, r_lim, r_rate], 1), extra], 1) * self.step_dt
+    self.finished_sums.copy_(torch.where(done.unsqueeze(1), sums, self.finished_sums))
+    self.episode_sums.copy_(torch.where(done.unsqueeze(1), 0.0, sums))
+    self.last_action.copy_(action)
     # partial reset + forward (manager_based_rl_env.py:128-132), mask-based: no host sync; the curriculum runs
     # before the reset events (_reset_idx, :205-208)
     if self.terrain_curriculum:

@@ -44,6 +44,9 @@ class B2Stats(ctypes.Structure):
   ]
 
 
+VELENV_NTERM = 14  # B2_VELENV_NTERM: reward terms with an episode sum
+
+
 class B2VelEnvArgs(ctypes.Structure):
   _fields_ = (
     [(n, ctypes.c_void_p) for n in (
@@ -55,6 +58,15 @@ class B2VelEnvArgs(ctypes.Structure):
     + [(n, ctypes.c_void_p) for n in ("terrain_origins", "terrain_levels", "terrain_types", "terrain_level_mean")]
     + [(n, ctypes.c_float) for n in ("move_up_dist", "episode_length_s")]
     + [(n, ctypes.c_int32) for n in ("rows", "cols", "curriculum")]
+    + [("weight", ctypes.c_float * (VELENV_NTERM - 5))]
+    + [(n, ctypes.c_float) for n in (
+      "air_threshold_min", "air_threshold_max", "air_command_threshold", "air_command_scale_width",
+      "clearance_target_height", "clearance_std", "clearance_tanh_mult")]
+    + [(n, ctypes.c_int32) for n in ("air_continuous", "air_hard_scale", "n_air", "n_slide", "n_clear", "root_body")]
+    + [(n, ctypes.c_void_p) for n in (
+      "air_sensor_adr", "slide_sensor_adr", "slide_geom", "slide_body", "clear_geom", "clear_body", "air_time",
+      "contact_time", "last_air_time", "episode_sums", "finished_sums")]
+    + [("rewards", ctypes.c_int32)]
   )
 
 
