@@ -114,6 +114,7 @@ int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_ho
  * tasks/velocity/velocity_env_cfg.py, as two launches. All pointers are device pointers. */
 #define B2_VELENV_NU(nu) (16 + 9 + 2 * (nu))
 #define B2_VELENV_NTERM 14 /* reward terms with an episode sum (B2VelEnvArgs.rewards) */
+#define B2_VELENV_NSTAGE 8 /* stages of the command-velocity curriculum (B2VelEnvArgs.n_stage) */
 typedef struct B2VelEnvArgs {
   const float* action;            /* [n][nu] */
   const float* U;                 /* [n][B2_VELENV_NU(nu)] uniforms in [0,1): 0-1 reset xy, 2 yaw, 3-5 command, 6 heading
@@ -183,6 +184,36 @@ typedef struct B2VelEnvArgs {
   float* episode_sums;            /* [n][B2_VELENV_NTERM] in/out, or null */
   float* finished_sums;           /* [n][B2_VELENV_NTERM] out: the sums of the episode a done env just ended */
   int32_t rewards;
+  /* the command term as the reference's tasks configure it (UniformVelocityCommandCfg,
+   * tasks/velocity/mdp/velocity_command.py:179-203), the command-velocity curriculum (commands_vel,
+   * tasks/velocity/mdp/curriculums.py:55-74), per-joint posture widths (posture, envs/mdp/rewards.py:73-104) and the
+   * command's metrics (velocity_command.py:43-62).  Each part is off when its fields are zero or null:
+   *   command = 0: the ranges x +-1, y +-0.5, yaw +-1, heading +-pi, stiffness 0.5, 10 % standing, timer 3..8 s
+   *     (b2_velenv_post writes them into the fields below).  A component is drawn as mid + (2u - 1) half (one IEEE
+   *     product and one IEEE sum), the timer as resample_lo + resample_span u, standing as u <= rel_standing; the
+   *     heading command is clamp(heading_stiffness wrap(target - heading), ang_lo, ang_hi).
+   *   n_stage > 0: counter = *step_counter + 1 is the step's common_step_counter; the lin_vel_x and ang_vel_z ranges
+   *     of the step are those of the last stage s in list order with stage_step[s] < counter (the cfg's when none
+   *     is).  b2_velenv_post advances *step_counter after the post kernel (one one-thread launch).
+   *   posture_inv_std2: the pose term is exp(-mean_j(d_j^2 / std_j^2)); null: exp(-mean_j(d_j^2) / 0.09).
+   *   metric_xy: every env adds |cmd_xy - v_b,xy| / metric_steps and |cmd_z - w_b,z| / metric_steps, from the command
+   *     before this step's timer resample and the post-physics velocity.  A done env first moves its sums to
+   *     finished_metrics and restarts them at 0; its first increment uses the fresh draw (before heading control and
+   *     standing) and the post-reset state.  Null skips the metrics. */
+  float cmd_mid[4], cmd_half[4];  /* lin_vel_x, lin_vel_y, ang_vel_z, heading: (lo + hi) / 2, (hi - lo) / 2 */
+  float ang_lo, ang_hi;           /* ang_vel_z range */
+  float heading_stiffness, rel_standing, resample_lo, resample_span;
+  int32_t command_cfg;
+  int32_t n_stage;                /* <= B2_VELENV_NSTAGE */
+  int32_t stage_step[B2_VELENV_NSTAGE];
+  float stage_mid[B2_VELENV_NSTAGE], stage_half[B2_VELENV_NSTAGE]; /* of the stage's range, as cmd_mid / cmd_half */
+  float stage_lo[B2_VELENV_NSTAGE], stage_hi[B2_VELENV_NSTAGE];
+  int32_t* step_counter;          /* [1] in/out: common_step_counter */
+  const float* posture_inv_std2;  /* [nu] 1 / std^2 per joint, or null */
+  float* metric_xy;               /* [n] in/out: error_vel_xy of the running command episode, or null */
+  float* metric_yaw;              /* [n] in/out: error_vel_yaw */
+  float* finished_metrics;        /* [n][2] out: (xy, yaw) of the episode a done env just ended */
+  float metric_steps;             /* resampling_time_range[1] / step_dt */
 } B2VelEnvArgs;
 int b2_velenv_pre(b2_sim* sim, const float* action, const float* default_joint_pos,
                   const float* action_scale, void* cuda_stream);

@@ -80,6 +80,18 @@ ACTION_SCALE = {n: 0.25 * a.effort_limit / a.stiffness for a in ACTUATORS for n 
 
 FOOT_GEOMS = [f"{s}_foot{i}_collision" for s in ("left", "right") for i in range(1, 8)]
 
+# posture reward widths per joint (tasks/velocity/config/g1/rough_env_cfg.py:51-69): {regex: std}
+POSTURE_STD = {
+  # lower body
+  r".*hip_pitch.*": 0.3, r".*hip_roll.*": 0.15, r".*hip_yaw.*": 0.15, r".*knee.*": 0.35, r".*ankle_pitch.*": 0.25,
+  r".*ankle_roll.*": 0.1,
+  # waist
+  r".*waist_yaw.*": 0.15, r".*waist_roll.*": 0.08, r".*waist_pitch.*": 0.1,
+  # arms
+  r".*shoulder_pitch.*": 0.35, r".*shoulder_roll.*": 0.15, r".*shoulder_yaw.*": 0.1, r".*elbow.*": 0.25,
+  r".*wrist.*": 0.3,
+}
+
 
 def velocity_sensors():
   # tasks/velocity/config/g1/rough_env_cfg.py:18-28

@@ -49,6 +49,8 @@ FULL_COLLISION = CollisionCfg(
 
 ACTION_SCALE = {n: 0.25 * a.effort_limit / a.stiffness for a in ACTUATORS for n in a.joint_names_expr}
 FOOT_GEOMS = [f"{leg}_foot_collision" for leg in ("FR", "FL", "RR", "RL")]
+# posture reward widths per joint (tasks/velocity/config/go1/rough_env_cfg.py:39-42): {regex: std}
+POSTURE_STD = {r".*(FR|FL|RR|RL)_(hip|thigh)_joint.*": 0.3, r".*(FR|FL|RR|RL)_calf_joint.*": 0.6}
 
 
 def velocity_sensors():

@@ -5,7 +5,8 @@
 //   post : episode counter, terminations (bad_orientation, time_out), rewards (the five fixed terms, the opt-in terms
 //          of B2VelEnvArgs.rewards and their episode sums), the terrain-level curriculum of
 //          the reset envs (opt-in, curriculums.py:18-52), masked reset (events.py:43-124), interval push
-//          (events.py:127-143), command resample, observations.
+//          (events.py:127-143), command resample (configurable ranges, the opt-in command-velocity curriculum and
+//          the command's metrics), observations.
 // The torch implementation in mjlab_b200/envs/velocity_env.py is the reference; both consume the same
 // per-step uniform numbers U[n][B2_VELENV_NU(nu)] (layout in include/b2sim.h) so they can be compared on one state
 // (tests/test_mdp_kernels.py).
@@ -130,6 +131,16 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   float htarget = A.heading_target[w];
   bool standing = A.is_standing[w] != 0;
   const float v0 = qvel[0], v1 = qvel[1], v2 = qvel[2], wz = qvel[5];
+  // ranges of lin_vel_x and ang_vel_z in this step: the cfg's, or the last curriculum stage the counter has passed
+  float xm = A.cmd_mid[0], xh = A.cmd_half[0], zm = A.cmd_mid[2], zh = A.cmd_half[2], zlo = A.ang_lo, zhi = A.ang_hi;
+  if (A.n_stage > 0) {
+    const int counter = *A.step_counter + 1;
+#pragma unroll
+    for (int s = 0; s < B2_VELENV_NSTAGE; s++)
+      if (s < A.n_stage && counter > A.stage_step[s]) {
+        xm = zm = A.stage_mid[s]; xh = zh = A.stage_half[s]; zlo = A.stage_lo[s]; zhi = A.stage_hi[s];
+      }
+  }
   b2e_rot_inv(q, down, gb);
   bool term = acosf(fminf(fmaxf(-gb[2], -1.f), 1.f)) > A.fall_angle;  // bad_orientation
   bool trunc = ep >= A.max_episode_length;                              // time_out
@@ -138,15 +149,17 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   b2e_rot_inv(q, lin, lb);
   float e0 = c0 - lb[0], e1 = c1 - lb[1], e2 = c2 - wz;
   float r_lin = expf(-(e0 * e0 + e1 * e1) / 0.25f), r_ang = expf(-(e2 * e2) / 0.25f);
-  float pose = 0.f, lim = 0.f, rate = 0.f;
+  float pose = 0.f, wpose = 0.f, lim = 0.f, rate = 0.f;
+  const float* inv_std2 = A.posture_inv_std2;  // per-joint widths: wpose; the single width keeps its own sum
   for (int a = lane; a < nu; a += 32) {
     float jp = qpos[7 + a], dj = jp - A.default_joint_pos[a];
     pose += dj * dj;
+    if (inv_std2) wpose += dj * dj * inv_std2[a];
     lim += fmaxf(A.soft_lo[a] - jp, 0.f) + fmaxf(jp - A.soft_hi[a], 0.f);
     float da = act[a] - last[a];
     rate += da * da;
   }
-  pose = b2e_wsum(pose); lim = b2e_wsum(lim); rate = b2e_wsum(rate);
+  pose = b2e_wsum(inv_std2 ? wpose : pose); lim = b2e_wsum(lim); rate = b2e_wsum(rate);
   bool done = term || trunc;
   // opt-in terms (B2VelEnvArgs.rewards): r[i] is term 5 + i unweighted, evaluated only at a non-zero weight
   float r[B2_VELENV_NTERM - 5] = {}, extra = 0.f;
@@ -202,7 +215,7 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     }
   }
   __syncwarp();  // every lane holds the pre-reset state it needs; writes may start
-  float r_pose = expf(-(pose / (float)nu) / 0.09f);
+  float r_pose = inv_std2 ? expf(-(pose / (float)nu)) : expf(-(pose / (float)nu) / 0.09f);
   const float fixed = r_lin + r_ang + r_pose - lim - 0.1f * rate;
   const float reward = any ? (fixed + extra) * A.step_dt : fixed * A.step_dt;
   if (lane == 0) {
@@ -247,21 +260,40 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     for (int a = lane; a < nu; a += 32) last[a] = act[a];
   }
   // command term (CommandTerm.compute + UniformVelocityCommand, velocity_command.py:64-110): resample on
-  // reset and when the timer runs out, then heading control and standing envs every step
+  // reset and when the timer runs out, then heading control and standing envs every step.  mid + (2u - 1) half
+  // is rounded as written (no contraction), so that at the default ranges it is bit-identical to 2u - 1, u - 0.5 and
+  // (2u - 1) pi (scaling by 2 is exact)
+  const float o0 = c0, o1 = c1, o2 = c2;  // the command before this step's resample (metrics)
   if (done || ctl <= 0.f) {
-    c0 = U[3] * 2.f - 1.f; c1 = U[4] - 0.5f; c2 = U[5] * 2.f - 1.f;
-    htarget = (U[6] * 2.f - 1.f) * 3.14159265358979f;
-    standing = U[7] <= 0.1f;
-    ctl = 3.f + 5.f * U[8];
+    c0 = b2e_add_rn(xm, b2e_mul_rn(U[3] * 2.f - 1.f, xh));
+    c1 = b2e_add_rn(A.cmd_mid[1], b2e_mul_rn(U[4] * 2.f - 1.f, A.cmd_half[1]));
+    c2 = b2e_add_rn(zm, b2e_mul_rn(U[5] * 2.f - 1.f, zh));
+    htarget = b2e_add_rn(A.cmd_mid[3], b2e_mul_rn(U[6] * 2.f - 1.f, A.cmd_half[3]));
+    standing = U[7] <= A.rel_standing;
+    ctl = A.resample_lo + A.resample_span * U[8];
   }
   __syncwarp();  // the reset state is visible to every lane
   {
     // heading_w = atan2 of the body x axis in the world (entity/data.py:480-484), from the post-reset pose
     float qw = qpos[3], qx = qpos[4], qy = qpos[5], qz = qpos[6];
+    if (A.metric_xy && lane == 0) {
+      // metrics (CommandTerm.reset, then _update_metrics in compute): a done env hands its sums over and restarts;
+      // the increment takes the fresh draw of a done env and every other env's command from before the resample,
+      // with the velocity of the post-reset state (before the push)
+      float qq[4] = {qw, qx, qy, qz}, vw[3] = {qvel[0], qvel[1], qvel[2]}, vb[3];
+      b2e_rot_inv(qq, vw, vb);
+      const float ex = (done ? c0 : o0) - vb[0], ey = (done ? c1 : o1) - vb[1];
+      const float exy = sqrtf(ex * ex + ey * ey) / A.metric_steps;
+      const float eyaw = fabsf((done ? c2 : o2) - qvel[5]) / A.metric_steps;
+      const float mxy = A.metric_xy[w], myaw = A.metric_yaw[w];
+      if (done) { A.finished_metrics[2 * (size_t)w] = mxy; A.finished_metrics[2 * (size_t)w + 1] = myaw; }
+      A.metric_xy[w] = (done ? 0.f : mxy) + exy;
+      A.metric_yaw[w] = (done ? 0.f : myaw) + eyaw;
+    }
     float fx = 1.f - 2.f * (qy * qy + qz * qz), fy = 2.f * (qx * qy + qw * qz);
     float err = htarget - atan2f(fy, fx);
     err -= 6.28318530717959f * floorf((err + 3.14159265358979f) / 6.28318530717959f);  // wrap_to_pi
-    c2 = fminf(fmaxf(0.5f * err, -1.f), 1.f);
+    c2 = fminf(fmaxf(A.heading_stiffness * err, zlo), zhi);
     if (standing) { c0 = 0.f; c1 = 0.f; c2 = 0.f; }
   }
   // interval event: push_by_setting_velocity
@@ -308,6 +340,10 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     o[9 + 2 * nu + a] = la;
   }
 }
+
+// common_step_counter += 1 after the post kernel, launched only with the command-velocity curriculum on: the post
+// kernel's warps all read the counter, so none of them can advance it.
+__global__ void b2_velenv_counter_kernel(int32_t* __restrict__ counter) { *counter += 1; }
 
 // Mean terrain level after the post kernel's curriculum update, the value terrain_levels_vel returns for logging: one
 // CTA, launched only when the curriculum is on.  The sum of integer levels is exact in any order, so no accumulator

@@ -1107,11 +1107,29 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
       return fail("b2_velenv_post: the reward terms need at most 32 feet each, a valid root_body, the arrays of "
                   "every term with a non-zero weight, and finished_sums beside episode_sums");
   }
+  if (args->command_cfg && !(args->resample_lo > 0.f && args->resample_span >= 0.f && args->ang_lo <= args->ang_hi))
+    return fail("b2_velenv_post: the command needs resample_lo > 0, resample_span >= 0 and ang_lo <= ang_hi");
+  if (args->n_stage < 0 || args->n_stage > B2_VELENV_NSTAGE || (args->n_stage > 0 && !args->step_counter))
+    return fail("b2_velenv_post: the command curriculum needs 0 <= n_stage <= B2_VELENV_NSTAGE and a step_counter");
+  if (args->metric_xy && (!args->metric_yaw || !args->finished_metrics || !(args->metric_steps > 0.f)))
+    return fail("b2_velenv_post: the command metrics need metric_yaw, finished_metrics and metric_steps > 0");
+  B2VelEnvArgs a = *args;
+  if (!a.command_cfg) {  // the ranges, widths and timer of velocity_env_cfg.py:66-83
+    const float mid[4] = {0.f, 0.f, 0.f, 0.f}, half[4] = {1.f, 0.5f, 1.f, 3.14159265358979f};
+    for (int k = 0; k < 4; k++) { a.cmd_mid[k] = mid[k]; a.cmd_half[k] = half[k]; }
+    a.ang_lo = -1.f; a.ang_hi = 1.f;
+    a.heading_stiffness = 0.5f; a.rel_standing = 0.1f; a.resample_lo = 3.f; a.resample_span = 5.f;
+  }
   DeviceGuard guard(s->device);
   b2_velenv_post_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(  // one warp per environment
-      s->hd, s->hm.nq, s->hm.nv, s->hm.nu, *args);
+      s->hd, s->hm.nq, s->hm.nv, s->hm.nu, a);
   s->launches++;
   CUDA_OK(cudaGetLastError());
+  if (a.n_stage > 0) {
+    b2_velenv_counter_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(a.step_counter);
+    s->launches++;
+    CUDA_OK(cudaGetLastError());
+  }
   if (args->curriculum) {
     b2_velenv_level_mean_kernel<<<1, kLevelMeanThreads, 0, (cudaStream_t)stream>>>(
         s->nworld, args->terrain_levels, args->terrain_level_mean);

@@ -62,6 +62,36 @@ class VelocityRewardsCfg:
 
 
 @dataclass
+class VelocityCommandCfg:
+  """The task's UniformVelocityCommandCfg (velocity_env_cfg.py:66-83, tasks/velocity/mdp/velocity_command.py:179-203):
+  (lo, hi) ranges of the commanded body-frame velocities and the heading target, the heading controller's gain, the
+  share of standing envs (zero command) and the resampling timer in seconds.  Every env is a heading env
+  (rel_heading_envs 1) and none starts at its command's velocity (init_velocity_prob 0), as in all of the reference's
+  velocity tasks."""
+
+  lin_vel_x: tuple = (-1.0, 1.0)
+  lin_vel_y: tuple = (-0.5, 0.5)
+  ang_vel_z: tuple = (-1.0, 1.0)
+  heading: tuple = (-math.pi, math.pi)
+  heading_control_stiffness: float = 0.5
+  rel_standing_envs: float = 0.1
+  resampling_time_range: tuple = (3.0, 8.0)
+
+  def __post_init__(self):
+    self.check()
+
+  def check(self) -> None:
+    for k in ("lin_vel_x", "lin_vel_y", "ang_vel_z", "heading", "resampling_time_range"):
+      lo, hi = getattr(self, k)
+      if not lo <= hi:
+        raise ValueError(f"command {k}: lo {lo} > hi {hi}")
+    if not 0.0 <= self.rel_standing_envs <= 1.0:
+      raise ValueError(f"command rel_standing_envs must lie in [0, 1], not {self.rel_standing_envs}")
+    if not self.resampling_time_range[0] > 0.0:
+      raise ValueError(f"command resampling_time_range must be positive, not {self.resampling_time_range}")
+
+
+@dataclass
 class VelocityEnvCfg:
   robot: str = "g1"
   num_envs: int = 4096
@@ -86,6 +116,64 @@ class VelocityEnvCfg:
     )
   )
   rewards: VelocityRewardsCfg = field(default_factory=VelocityRewardsCfg)  # opt-in terms beside the fixed five
+  command: VelocityCommandCfg = field(default_factory=VelocityCommandCfg)
+  # command-velocity curriculum (commands_vel, tasks/velocity/mdp/curriculums.py:55-74): (step, (lo, hi)) stages; in
+  # a step, lin_vel_x and ang_vel_z take the range of the last stage in list order whose step is below the step's
+  # common_step_counter.  Empty: off
+  command_curriculum: tuple = ()
+  # per-joint widths of the posture reward (posture, envs/mdp/rewards.py:73-104): {joint regex: std}, every joint
+  # matched by exactly one pattern and every pattern by some joint.  None: one width of 0.3 for every joint
+  posture_std: dict | None = None
+
+
+def _float32(x) -> float:
+  return float(np.float32(x))
+
+
+def _mid_half(lo: float, hi: float) -> tuple[float, float]:
+  """A range as the kernel draws it, mid + (2u - 1) half, in fp32."""
+  return _float32((lo + hi) / 2), _float32((hi - lo) / 2)
+
+
+# the reference's velocity tasks with a model here (tasks/velocity/config/*/__init__.py), as their cfg classes set them
+# (UnitreeG1FlatEnvCfg, UnitreeGo1FlatEnvCfg, UnitreeGo1RoughEnvCfg; the command curriculum of velocity_env_cfg.py:232-241)
+_GO1_COMMAND_STAGES = ((500 * 24, (-3.0, 3.0)),)
+VELOCITY_TASKS = {
+  "Mjlab-Velocity-Flat-Unitree-G1": dict(robot="g1", terrain="flat", push_vel=0.5, posture_std=g1.POSTURE_STD),
+  "Mjlab-Velocity-Flat-Unitree-Go1": dict(robot="go1", terrain="flat", push_vel=1.0, posture_std=go1.POSTURE_STD,
+                                          command_curriculum=_GO1_COMMAND_STAGES),
+  "Mjlab-Velocity-Rough-Unitree-Go1": dict(robot="go1", terrain="rough", terrain_curriculum=True, push_vel=1.0,
+                                           posture_std=go1.POSTURE_STD, command_curriculum=_GO1_COMMAND_STAGES),
+}
+
+
+def velocity_task_cfg(name: str, **overrides) -> VelocityEnvCfg:
+  """The VelocityEnvCfg of one of the reference's velocity tasks by its registered name, with `overrides` (any
+  VelocityEnvCfg field, e.g. num_envs) on top."""
+  if name not in VELOCITY_TASKS:
+    raise ValueError(f"unknown velocity task {name!r}; known: {', '.join(VELOCITY_TASKS)}")
+  preset = dict(VELOCITY_TASKS[name])
+  preset["posture_std"] = dict(preset["posture_std"])
+  return VelocityEnvCfg(**{**preset, **overrides})
+
+
+def resolve_posture_std(posture_std: dict, joint_names: list[str]) -> list[float]:
+  """One std per joint from {regex: std}, by resolve_matching_names_values' rules (re.fullmatch): a joint matched by
+  two patterns or by none, or a pattern that matches no joint, is a ValueError."""
+  out = []
+  used = set()
+  for j in joint_names:
+    hits = [p for p in posture_std if re.fullmatch(p, j)]
+    if len(hits) != 1:
+      raise ValueError(f"posture_std: joint '{j}' is matched by {len(hits)} patterns {hits}, not exactly one")
+    used.add(hits[0])
+    out.append(float(posture_std[hits[0]]))
+  unused = [p for p in posture_std if p not in used]
+  if unused:
+    raise ValueError(f"posture_std: patterns {unused} match no joint")
+  if not all(v > 0.0 for v in out):
+    raise ValueError("posture_std: every std must be positive")
+  return out
 
 
 def _resolve(pattern_map: dict, names: list[str], default: float) -> list[float]:
@@ -182,6 +270,7 @@ class VelocityFlatEnv:
     lo_t, hi_t = cfg.push_interval_s
     self.push_time_left.copy_(self._rand(n) * (hi_t - lo_t) + lo_t)
     self._init_rewards()
+    self._init_command(jnames)
     if self.native_mdp:
       self._init_native()
     self._reset_all(curriculum=False)  # no episode has ended yet: the initial levels stand
@@ -251,6 +340,61 @@ class VelocityFlatEnv:
     self.episode_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
     self.finished_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
 
+  def _init_command(self, joint_names: list[str]) -> None:
+    """The command's ranges in fp32 as the kernel draws them, the curriculum's stage table and counter, the posture
+    widths, and the command's metrics."""
+    cfg, n, dev = self.cfg, self.num_envs, self.device
+    cc = cfg.command
+    cc.check()
+    self._cmd_mid_half = [_mid_half(*getattr(cc, k)) for k in ("lin_vel_x", "lin_vel_y", "ang_vel_z", "heading")]
+    stages = list(cfg.command_curriculum)
+    if len(stages) > 8:
+      raise ValueError(f"command_curriculum: at most 8 stages, got {len(stages)}")
+    for step, (lo, hi) in stages:
+      if int(step) != step or not 0 <= step < 2 ** 31 or not lo <= hi:
+        raise ValueError(f"command_curriculum: stage ({step}, ({lo}, {hi})) needs an integer step in [0, 2^31) and "
+                         "lo <= hi")
+    f32 = dict(dtype=torch.float32, device=dev)
+    # (mid, half, lo, hi) of lin_vel_x and ang_vel_z as configured, and of each stage
+    self._cmd_base = torch.tensor([[*self._cmd_mid_half[k], *getattr(cc, r)] for k, r in ((0, "lin_vel_x"),
+                                                                                        (2, "ang_vel_z"))], **f32)
+    self._stages = [(int(st), *_mid_half(lo, hi), _float32(lo), _float32(hi)) for st, (lo, hi) in stages]
+    self._stage_step = torch.tensor([st[0] for st in self._stages], dtype=torch.int32, device=dev)
+    self._stage_vals = torch.tensor([st[1:] for st in self._stages], **f32).reshape(-1, 4)
+    # common_step_counter (manager_based_rl_env.py:117); it only advances with the command curriculum on, the one
+    # thing that reads it
+    self.common_step_counter = torch.zeros(1, dtype=torch.int32, device=dev)
+    self.posture_inv_std2 = None
+    if cfg.posture_std is not None:
+      std = np.asarray(resolve_posture_std(cfg.posture_std, joint_names), dtype=np.float64)
+      self.posture_inv_std2 = torch.tensor(1.0 / std ** 2, **f32)
+    self.metric_steps = _float32(cc.resampling_time_range[1] / self.step_dt)
+    self.metric_xy = torch.zeros(n, **f32)
+    self.metric_yaw = torch.zeros(n, **f32)
+    self.finished_metrics = torch.zeros(n, 2, **f32)
+
+  def _command_ranges(self, counter: torch.Tensor):
+    """[2, 4] (mid, half, lo, hi) of lin_vel_x and ang_vel_z at common_step_counter `counter`: those of the last stage
+    in list order whose step is below it, or the cfg's (commands_vel, curriculums.py:55-74, which writes the stage's
+    range into the cfg for good)."""
+    if not self._stages:
+      return self._cmd_base
+    idx = torch.arange(len(self._stages), device=self.device)
+    last = torch.where(counter > self._stage_step, idx, -1).max()
+    return torch.where(last >= 0, self._stage_vals[last.clamp(min=0)], self._cmd_base)
+
+  def command_log(self) -> dict:
+    """``Metrics/twist/error_vel_xy`` and ``error_vel_yaw`` of CommandManager.reset (managers/command_manager.py:128-134,
+    velocity_command.py:43-62) for the envs whose episode ended in the last step: the mean of their accumulated errors
+    (NaN when none ended); with the command curriculum on also ``Curriculum/command_vel``, the upper lin_vel_x bound in
+    effect.  Device tensors, no host synchronisation."""
+    done = self._done_buf.unsqueeze(1)
+    mean = torch.where(done, self.finished_metrics, 0.0).sum(0) / done.sum()
+    out = {"Metrics/twist/error_vel_xy": mean[0], "Metrics/twist/error_vel_yaw": mean[1]}
+    if self._stages:
+      out["Curriculum/command_vel"] = self._command_ranges(self.common_step_counter)[0, 3]
+    return out
+
   def reward_log(self) -> dict:
     """``Episode_Reward/<term>`` of RewardManager.reset (managers/reward_manager.py:61-75) for the envs whose episode
     ended in the last step: the mean of their episode sums over episode_length_s (NaN when none ended), for the fixed
@@ -313,6 +457,24 @@ class VelocityFlatEnv:
     a.air_continuous, a.air_hard_scale = rc.reward_mode == "continuous", rc.command_scale_type == "hard"
     a.n_air, a.n_slide, a.n_clear = len(self._air_adr), len(self._slide_adr), len(self._clear_geom)
     a.root_body, a.rewards = self._root_body, 1
+    cc = self.cfg.command
+    for k, (mid, half) in enumerate(self._cmd_mid_half):
+      a.cmd_mid[k], a.cmd_half[k] = mid, half
+    a.ang_lo, a.ang_hi = cc.ang_vel_z
+    a.heading_stiffness, a.rel_standing = cc.heading_control_stiffness, cc.rel_standing_envs
+    lo_t, hi_t = cc.resampling_time_range
+    a.resample_lo, a.resample_span = lo_t, _float32(np.float32(hi_t) - np.float32(lo_t))
+    a.command_cfg = 1
+    a.n_stage = len(self._stages)
+    for s, (step, mid, half, lo, hi) in enumerate(self._stages):
+      a.stage_step[s], a.stage_mid[s], a.stage_half[s], a.stage_lo[s], a.stage_hi[s] = step, mid, half, lo, hi
+    for name, t in (("step_counter", self.common_step_counter), ("posture_inv_std2", self.posture_inv_std2),
+                    ("metric_xy", self.metric_xy), ("metric_yaw", self.metric_yaw),
+                    ("finished_metrics", self.finished_metrics)):
+      if t is not None:
+        assert t.is_contiguous()
+        setattr(a, name, t.data_ptr())
+    a.metric_steps = self.metric_steps
     self._native_args = a
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
@@ -403,22 +565,49 @@ class VelocityFlatEnv:
         out[:, i] = f()
     return out * torch.tensor(W, device=self.device)
 
-  def _update_command(self, done: torch.Tensor, U: torch.Tensor) -> None:
-    """CommandTerm.compute + UniformVelocityCommand (tasks/velocity/mdp/velocity_command.py:64-110): resample on
-    reset and on timer expiry (3..8 s), heading control on every env, standing envs (10 %) get a zero command."""
+  def _posture(self, jp: torch.Tensor) -> torch.Tensor:
+    """The pose reward (posture, envs/mdp/rewards.py:73-104): exp(-mean(d^2 / std^2)) with the per-joint widths of
+    posture_std, else exp(-mean(d^2) / 0.3^2)."""
+    d2 = (jp - self.default_joint_pos) ** 2
+    if self.posture_inv_std2 is None:
+      return torch.exp(-d2.mean(1) / 0.09)
+    return torch.exp(-(d2 * self.posture_inv_std2).mean(1))
+
+  def _update_command(self, done: torch.Tensor, U: torch.Tensor, metrics: bool = True) -> None:
+    """CommandTerm.compute + UniformVelocityCommand (tasks/velocity/mdp/velocity_command.py:43-110): resample on
+    reset and on timer expiry, heading control on every env, standing envs get a zero command.  A component is drawn
+    as mid + (2u - 1) half.  With `metrics`, the command's error metrics first take this step's increment (a done env
+    hands its sums over and restarts them)."""
+    cc = self.cfg.command
+    rng = self._command_ranges(self.common_step_counter)
+    (ym, yh), (hm, hh) = self._cmd_mid_half[1], self._cmd_mid_half[3]
     ctl = self.cmd_time_left - self.step_dt
     rs = done | (ctl <= 0)
-    cmd = torch.stack([U[:, 3] * 2 - 1, U[:, 4] - 0.5, U[:, 5] * 2 - 1], dim=1)
+    cmd = torch.stack([rng[0, 0] + (U[:, 3] * 2 - 1) * rng[0, 1], ym + (U[:, 4] * 2 - 1) * yh,
+                       rng[1, 0] + (U[:, 5] * 2 - 1) * rng[1, 1]], dim=1)
+    old = self.command.clone()
     self.command.copy_(torch.where(rs.unsqueeze(1), cmd, self.command))
-    self.heading_target.copy_(torch.where(rs, (U[:, 6] * 2 - 1) * math.pi, self.heading_target))
-    self.is_standing.copy_(torch.where(rs, U[:, 7] <= 0.1, self.is_standing))
-    self.cmd_time_left.copy_(torch.where(rs, 3.0 + 5.0 * U[:, 8], ctl))
+    self.heading_target.copy_(torch.where(rs, hm + (U[:, 6] * 2 - 1) * hh, self.heading_target))
+    self.is_standing.copy_(torch.where(rs, U[:, 7] <= _float32(cc.rel_standing_envs), self.is_standing))
+    lo_t, hi_t = cc.resampling_time_range
+    span = _float32(np.float32(hi_t) - np.float32(lo_t))
+    self.cmd_time_left.copy_(torch.where(rs, lo_t + span * U[:, 8], ctl))
     q = self.sim.data.qpos[:, 3:7]
+    if metrics:  # _update_metrics (velocity_command.py:49-62) after CommandTerm.reset of the done envs
+      d = self.sim.data
+      m = torch.where(done.unsqueeze(1), cmd, old)
+      vb = quat_rotate_inverse(q, d.qvel[:, 0:3])
+      exy = (m[:, :2] - vb[:, :2]).norm(dim=1) / self.metric_steps
+      eyaw = (m[:, 2] - d.qvel[:, 5]).abs() / self.metric_steps
+      self.finished_metrics.copy_(torch.where(done.unsqueeze(1), torch.stack([self.metric_xy, self.metric_yaw], 1),
+                                              self.finished_metrics))
+      self.metric_xy.copy_(torch.where(done, 0.0, self.metric_xy) + exy)
+      self.metric_yaw.copy_(torch.where(done, 0.0, self.metric_yaw) + eyaw)
     fx = 1 - 2 * (q[:, 2] ** 2 + q[:, 3] ** 2)
     fy = 2 * (q[:, 1] * q[:, 2] + q[:, 0] * q[:, 3])
     err = self.heading_target - torch.atan2(fy, fx)
     err = err - 2 * math.pi * torch.floor((err + math.pi) / (2 * math.pi))
-    self.command[:, 2] = (0.5 * err).clamp(-1.0, 1.0)
+    self.command[:, 2] = torch.minimum(torch.maximum(cc.heading_control_stiffness * err, rng[1, 2]), rng[1, 3])
     self.command.copy_(torch.where(self.is_standing.unsqueeze(1), torch.zeros_like(self.command), self.command))
 
   def observations(self, U: torch.Tensor | None = None):
@@ -444,6 +633,8 @@ class VelocityFlatEnv:
   def _reset_all(self, curriculum: bool):
     all_ = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
     self.finished_sums.copy_(self.episode_sums)  # RewardManager.reset of every env
+    self.finished_metrics.copy_(torch.stack([self.metric_xy, self.metric_yaw], 1))  # CommandTerm.reset of every env
+    self.metric_xy.zero_(); self.metric_yaw.zero_()
     for t in (self.episode_sums, self.air_time, self.contact_time, self.last_air_time):
       t.zero_()
     U = self._draw()
@@ -451,7 +642,7 @@ class VelocityFlatEnv:
       self._terrain_curriculum(all_, U)
     self._reset_where(all_, U)
     self.sim.forward()
-    self._update_command(all_, U)
+    self._update_command(all_, U, metrics=False)
     return self.observations()
 
   def enable_cuda_graph(self) -> None:
@@ -526,6 +717,8 @@ class VelocityFlatEnv:
     two on one state)."""
     cfg, d = self.cfg, self.sim.data
     self.episode_length_buf += 1
+    if self._stages:
+      self.common_step_counter += 1
     q = d.qpos[:, 3:7]
     grav_b = quat_rotate_inverse(q, self._down)
     terminated = torch.acos((-grav_b[:, 2]).clamp(-1.0, 1.0)) > cfg.fall_angle  # bad_orientation
@@ -535,7 +728,7 @@ class VelocityFlatEnv:
     r_lin = torch.exp(-((self.command[:, :2] - lin_b[:, :2]) ** 2).sum(1) / 0.25)
     r_ang = torch.exp(-((self.command[:, 2] - d.qvel[:, 5]) ** 2) / 0.25)
     jp = d.qpos[:, 7:]
-    r_pose = torch.exp(-((jp - self.default_joint_pos) ** 2).mean(1) / 0.09)
+    r_pose = self._posture(jp)
     r_lim = -((self.soft_lo - jp).clamp(min=0) + (jp - self.soft_hi).clamp(min=0)).sum(1)
     r_rate = -0.1 * ((action - self.last_action) ** 2).sum(1)
     done = terminated | truncated

@@ -45,6 +45,7 @@ class B2Stats(ctypes.Structure):
 
 
 VELENV_NTERM = 14  # B2_VELENV_NTERM: reward terms with an episode sum
+VELENV_NSTAGE = 8  # B2_VELENV_NSTAGE: stages of the command-velocity curriculum
 
 
 class B2VelEnvArgs(ctypes.Structure):
@@ -67,6 +68,15 @@ class B2VelEnvArgs(ctypes.Structure):
       "air_sensor_adr", "slide_sensor_adr", "slide_geom", "slide_body", "clear_geom", "clear_body", "air_time",
       "contact_time", "last_air_time", "episode_sums", "finished_sums")]
     + [("rewards", ctypes.c_int32)]
+    + [(n, ctypes.c_float * 4) for n in ("cmd_mid", "cmd_half")]
+    + [(n, ctypes.c_float) for n in ("ang_lo", "ang_hi", "heading_stiffness", "rel_standing", "resample_lo",
+                                     "resample_span")]
+    + [(n, ctypes.c_int32) for n in ("command_cfg", "n_stage")]
+    + [("stage_step", ctypes.c_int32 * VELENV_NSTAGE)]
+    + [(n, ctypes.c_float * VELENV_NSTAGE) for n in ("stage_mid", "stage_half", "stage_lo", "stage_hi")]
+    + [(n, ctypes.c_void_p) for n in ("step_counter", "posture_inv_std2", "metric_xy", "metric_yaw",
+                                      "finished_metrics")]
+    + [("metric_steps", ctypes.c_float)]
   )
 
 
