@@ -273,7 +273,40 @@ typedef struct B2TrackEnvArgs {
                                      distribution this env step's draws used (1, p, b / nbins for one bin) */
   float adaptive_alpha, adaptive_uniform_ratio;
   int32_t nbins, adaptive, adaptive_kernel_size;
+  /* the task as a cfg class configures it (tracking_env_cfg.py:88-278, tasks/tracking/config/g1/flat_env_cfg.py) and
+   * the episode logs of its managers; task_cfg = 0 leaves every field below unread and runs the base task's literal
+   * terms (weights 0.5 0.5 1 1 1 1 -0.1 -10 -10, stds 0.3 0.4 0.3 0.4 1 3.14, thresholds 0.25 0.8 0.25, push from
+   * vel_range, both observation switches on) with no logs.  The RSI ranges are pose_range / vel_range above.
+   * Reward terms, in the order of the episode-sum columns (B2_TRACKENV_NREW): 0 motion_global_root_pos,
+   * 1 motion_global_root_ori, 2 motion_body_pos, 3 motion_body_ori, 4 motion_body_lin_vel, 5 motion_body_ang_vel
+   * (exp(-err / std2[i])), 6 action_rate_l2, 7 joint_limit, 8 self_collisions.  A term at weight 0 is not evaluated.
+   * reward = (sum of w_i r_i) step_dt; episode_sums[w][i] += w_i r_i step_dt.
+   * Terminations, in the order of term_flags (B2_TRACKENV_NTERM): 0 time_out, 1 anchor_pos, 2 anchor_ori,
+   * 3 ee_body_pos; term_on[k] = 0 removes term k + 1.  term_flags[w] holds every env's flags of this step.
+   * Motion errors (B2_TRACKENV_NMETRIC, commands.py:221-255): 0 anchor_pos, 1 anchor_rot, 2 anchor_lin_vel,
+   * 3 anchor_ang_vel, 4 body_pos, 5 body_rot, 6 body_lin_vel, 7 body_ang_vel (means of norms over the tracked bodies),
+   * 8 joint_pos, 9 joint_vel (norms over the joints).  An env that is not done takes them in post1 at its frame
+   * before the clip steps; a done env in post2, after the forward, at frame max(time_steps - 1, 0) against the
+   * relative targets of the previous post2.  A done env's episode_sums and motion_metrics rows move to finished_sums /
+   * finished_metrics in post1 (the episode sums restart at 0).
+   * policy_state_estimation = 0 drops motion_anchor_pos_b and base_lin_vel from the policy row ([n][5 nu + 9]); their
+   * noise columns of U are still drawn.  policy_corruption = 0 writes the policy terms without noise.  push_on = 0:
+   * no push, push_time_left untouched. */
+  int32_t task_cfg;
+  float weight[9], std2[6];       /* B2_TRACKENV_NREW weights; std^2 of reward terms 0-5 */
+  float term_threshold[3];        /* anchor_pos, anchor_ori, ee_body_pos */
+  int32_t term_on[3];
+  float push_range[12];           /* (lo, hi) x 6 of push_by_setting_velocity */
+  int32_t push_on, policy_state_estimation, policy_corruption;
+  float* episode_sums;            /* [n][B2_TRACKENV_NREW] in/out */
+  float* finished_sums;           /* [n][B2_TRACKENV_NREW] out */
+  float* term_flags;              /* [n][B2_TRACKENV_NTERM] out: 1 where the term fired this step */
+  float* motion_metrics;          /* [n][B2_TRACKENV_NMETRIC] in/out */
+  float* finished_metrics;        /* [n][B2_TRACKENV_NMETRIC] out */
 } B2TrackEnvArgs;
+#define B2_TRACKENV_NREW 9
+#define B2_TRACKENV_NTERM 4
+#define B2_TRACKENV_NMETRIC 10
 int b2_trackenv_post1(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
 int b2_trackenv_post2(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
 /* B2_START_ADAPTIVE only, between post1 and the masked forward (one CTA): metrics of the distribution post1 drew

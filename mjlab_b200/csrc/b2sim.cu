@@ -1153,6 +1153,18 @@ static int trackenv_check(b2_sim* s, const B2TrackEnvArgs* a) {
       (a->nbins < 1 || a->adaptive_kernel_size < 1 || !a->adaptive_kernel || !a->cdf || !a->bin_fail_ema ||
        !a->bin_fail_cur || !a->metrics))
     return fail("b2_trackenv: the adaptive sampler needs nbins >= 1, a kernel of size >= 1 and its five arrays");
+  if (a->task_cfg) {
+    bool ok = a->episode_sums && a->finished_sums && a->term_flags && a->motion_metrics && a->finished_metrics;
+    for (int k = 0; k < 6; k++) ok = ok && a->std2[k] > 0.f && a->std2[k] < INFINITY;
+    for (int k = 0; k < 3; k++)
+      ok = ok && (a->term_on[k] == 0 || (a->term_on[k] == 1 && a->term_threshold[k] > 0.f && a->term_threshold[k] < INFINITY));
+    for (int k = 0; k < 6; k++)
+      ok = ok && a->pose_range[2 * k] <= a->pose_range[2 * k + 1] && a->vel_range[2 * k] <= a->vel_range[2 * k + 1] &&
+           (!a->push_on || a->push_range[2 * k] <= a->push_range[2 * k + 1]);
+    if (!ok)
+      return fail("b2_trackenv: task_cfg needs the five log arrays, finite stds^2 > 0, finite thresholds > 0 on the "
+                  "terms that are on, and lo <= hi in every range");
+  }
   return 0;
 }
 int b2_trackenv_post1(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {

@@ -1,4 +1,6 @@
-from mjlab_b200.envs.tracking_env import TrackingEnvCfg, TrackingFlatEnv
+from mjlab_b200.envs.tracking_env import (TrackingEnvCfg, TrackingFlatEnv, TrackingRewardsCfg, TrackingTerminationsCfg,
+                                          tracking_task_cfg)
 from mjlab_b200.envs.velocity_env import VelocityCommandCfg, VelocityEnvCfg, VelocityFlatEnv, velocity_task_cfg
 
-__all__ = ["TrackingEnvCfg", "TrackingFlatEnv", "VelocityCommandCfg", "VelocityEnvCfg", "VelocityFlatEnv", "velocity_task_cfg"]
+__all__ = ["TrackingEnvCfg", "TrackingFlatEnv", "TrackingRewardsCfg", "TrackingTerminationsCfg", "VelocityCommandCfg",
+           "VelocityEnvCfg", "VelocityFlatEnv", "tracking_task_cfg", "velocity_task_cfg"]

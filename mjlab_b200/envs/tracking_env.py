@@ -44,6 +44,74 @@ BODY_NAMES = ("pelvis", "left_hip_roll_link", "left_knee_link", "left_ankle_roll
               "right_knee_link", "right_ankle_roll_link", "torso_link", "left_shoulder_roll_link", "left_elbow_link",
               "left_wrist_yaw_link", "right_shoulder_roll_link", "right_elbow_link", "right_wrist_yaw_link")  # g1/flat_env_cfg.py:26-41
 EE_NAMES = ("left_ankle_roll_link", "right_ankle_roll_link", "left_wrist_yaw_link", "right_wrist_yaw_link")  # :48-53
+# the columns of the episode logs (B2_TRACKENV_NREW / NTERM / NMETRIC of include/b2sim.h)
+TRACKING_TERMS = ("motion_global_root_pos", "motion_global_root_ori", "motion_body_pos", "motion_body_ori",
+                  "motion_body_lin_vel", "motion_body_ang_vel")
+REWARD_TERMS = TRACKING_TERMS + ("action_rate_l2", "joint_limit", "self_collisions")
+TERMINATION_TERMS = ("time_out", "anchor_pos", "anchor_ori", "ee_body_pos")
+METRICS = ("error_anchor_pos", "error_anchor_rot", "error_anchor_lin_vel", "error_anchor_ang_vel", "error_body_pos",
+           "error_body_rot", "error_body_lin_vel", "error_body_ang_vel", "error_joint_pos", "error_joint_vel")
+INT32_MAX = 2**31 - 1
+
+
+@dataclass
+class TrackingRewardsCfg:
+  """Weights and stds of the task's reward terms (tracking_env_cfg.py:201-252), the reference's defaults.  A term at
+  weight 0 is not evaluated and its episode sum stays 0 (reward_manager.py:82-84); it is still logged."""
+
+  motion_global_root_pos: float = 0.5
+  motion_global_root_ori: float = 0.5
+  motion_body_pos: float = 1.0
+  motion_body_ori: float = 1.0
+  motion_body_lin_vel: float = 1.0
+  motion_body_ang_vel: float = 1.0
+  action_rate_l2: float = -0.1
+  joint_limit: float = -10.0
+  self_collisions: float = -10.0
+  motion_global_root_pos_std: float = 0.3
+  motion_global_root_ori_std: float = 0.4
+  motion_body_pos_std: float = 0.3
+  motion_body_ori_std: float = 0.4
+  motion_body_lin_vel_std: float = 1.0
+  motion_body_ang_vel_std: float = 3.14
+
+  def check(self) -> None:
+    for t in TRACKING_TERMS:
+      s = getattr(self, t + "_std")
+      if not (math.isfinite(s) and s > 0.0):
+        raise ValueError(f"rewards {t}_std must be positive and finite, not {s}")
+    for t in REWARD_TERMS:
+      if not math.isfinite(getattr(self, t)):
+        raise ValueError(f"rewards {t}: the weight must be finite")
+
+
+@dataclass
+class TrackingTerminationsCfg:
+  """Thresholds of the task's termination terms (tracking_env_cfg.py:253-278): anchor_pos (bad_anchor_pos_z_only),
+  anchor_ori (bad_anchor_ori) and ee_body_pos (bad_motion_body_pos_z_only on EE_NAMES).  None removes a term;
+  time_out always stays."""
+
+  anchor_pos: float | None = 0.25
+  anchor_ori: float | None = 0.8
+  ee_body_pos: float | None = 0.25
+
+  def check(self) -> None:
+    for t in TERMINATION_TERMS[1:]:
+      v = getattr(self, t)
+      if v is not None and not (math.isfinite(v) and v > 0.0):
+        raise ValueError(f"terminations {t}: the threshold must be positive and finite (or None), not {v}")
+
+
+def _check_range6(name: str, r) -> None:
+  try:
+    pairs = [(float(lo), float(hi)) for lo, hi in r]
+  except (TypeError, ValueError):  # not a sequence of pairs of numbers
+    pairs = None
+  if pairs is None or len(pairs) != 6:
+    raise ValueError(f"{name} needs six (lo, hi) pairs (x, y, z, roll, pitch, yaw), got {r!r}")
+  for k, (lo, hi) in enumerate(pairs):
+    if not (math.isfinite(lo) and math.isfinite(hi) and lo <= hi):
+      raise ValueError(f"{name}[{k}]: ({lo}, {hi}) is not a finite range with lo <= hi")
 
 
 @dataclass
@@ -66,6 +134,59 @@ class TrackingEnvCfg:
   sim: SimulationCfg = field(
     default_factory=lambda: SimulationCfg(
       nconmax=150_000, njmax=250, mujoco=MujocoCfg(timestep=0.005, iterations=10, ls_iterations=20)))  # :283-291
+  rewards: TrackingRewardsCfg = field(default_factory=TrackingRewardsCfg)
+  terminations: TrackingTerminationsCfg = field(default_factory=TrackingTerminationsCfg)
+  pose_range: tuple = POSE_RANGE           # RSI offsets of the root pose, (lo, hi) of x, y, z, roll, pitch, yaw
+  velocity_range: tuple = VELOCITY_RANGE   # RSI offsets of the root velocity
+  push_velocity_range: tuple | None = VELOCITY_RANGE  # push_by_setting_velocity; None: no push event
+  policy_state_estimation: bool = True     # False: no motion_anchor_pos_b and no base_lin_vel in the policy group
+  policy_corruption: bool = True           # the policy group's enable_corruption
+  # per-episode logs of the reward, termination and command managers (reward_log, termination_log, command_log)
+  episode_logs: bool = False
+
+  def __post_init__(self):
+    self.check()
+
+  def check(self) -> None:
+    self.rewards.check()
+    self.terminations.check()
+    _check_range6("pose_range", self.pose_range)
+    _check_range6("velocity_range", self.velocity_range)
+    if self.push_velocity_range is not None:
+      _check_range6("push_velocity_range", self.push_velocity_range)
+    if not self.episode_length_s > 0:
+      raise ValueError(f"episode_length_s must be positive, not {self.episode_length_s}")
+
+  def is_base_task(self) -> bool:
+    """True when every task setting is the base task's (the fused kernels' literal terms) and no log is asked for."""
+    f = lambda r: None if r is None else tuple(tuple(float(x) for x in p) for p in r)
+    return (self.rewards == TrackingRewardsCfg() and self.terminations == TrackingTerminationsCfg()
+            and f(self.pose_range) == POSE_RANGE and f(self.velocity_range) == VELOCITY_RANGE
+            and f(self.push_velocity_range) == VELOCITY_RANGE and self.policy_state_estimation
+            and self.policy_corruption and not self.episode_logs)
+
+
+_NO_RSI = ((0.0, 0.0),) * 6  # an empty pose_range / velocity_range dict of MotionCommandCfg: every offset 0
+_PLAY = dict(policy_corruption=False, push_velocity_range=None, pose_range=_NO_RSI, velocity_range=_NO_RSI,
+             disable_adaptive_sampling=True, episode_length_s=int(1e9))
+# the reference's four G1 tracking tasks (tasks/tracking/config/g1/__init__.py), as their cfg classes set them
+# (G1FlatEnvCfg, G1FlatEnvCfg_PLAY, G1FlatNoStateEstimationEnvCfg, G1FlatNoStateEstimationEnvCfg_PLAY:
+# config/g1/flat_env_cfg.py), with the episode logs on
+TRACKING_TASKS = {
+  "Mjlab-Tracking-Flat-Unitree-G1": dict(),
+  "Mjlab-Tracking-Flat-Unitree-G1-Play": dict(_PLAY),
+  "Mjlab-Tracking-Flat-Unitree-G1-No-State-Estimation": dict(policy_state_estimation=False),
+  "Mjlab-Tracking-Flat-Unitree-G1-No-State-Estimation-Play": dict(_PLAY, policy_state_estimation=False),
+}
+
+
+def tracking_task_cfg(name: str, **overrides) -> TrackingEnvCfg:
+  """The TrackingEnvCfg of one of the reference's tracking tasks by its registered name, with `overrides` (any
+  TrackingEnvCfg field) on top.  As in the reference, whose robot cfg leaves it empty, the clip comes in as the
+  `motion_file` override (without one the env runs the synthetic clip)."""
+  if name not in TRACKING_TASKS:
+    raise ValueError(f"unknown tracking task {name!r}; known: {', '.join(TRACKING_TASKS)}")
+  return TrackingEnvCfg(**{"episode_logs": True, **TRACKING_TASKS[name], **overrides})
 
 
 def quat_inv(q):
@@ -111,7 +232,10 @@ class TrackingFlatEnv:
     f32 = dict(dtype=torch.float32, device=dev)
     self.nq, self.nv, self.nu = int(m.nq), int(m.nv), int(m.nu)
     self.step_dt = cfg.decimation * float(m.opt_timestep)
-    self.max_episode_length = math.ceil(cfg.episode_length_s / self.step_dt)
+    cfg.check()
+    # clamped to the episode counter's int32 range: an "effectively infinite" episode (the play tasks' 1e9 s) never
+    # truncates, on both paths, instead of wrapping to a negative limit
+    self.max_episode_length = min(math.ceil(cfg.episode_length_s / self.step_dt), INT32_MAX)
     self.gen = torch.Generator(device=dev)
     self.gen.manual_seed(cfg.seed)
     key = m.keys["robot/init_state"]
@@ -166,8 +290,9 @@ class TrackingFlatEnv:
     self.body_quat_relative_w = torch.zeros(n, nbk, 4, **f32)
     self._done_buf = torch.zeros(n, dtype=torch.bool, device=dev)
     self.log_row = torch.zeros(n, 3, **f32)  # (reward, terminated, truncated) for the rank-0 log gather
-    self._vr = torch.tensor(VELOCITY_RANGE, **f32)
-    self._pr = torch.tensor(POSE_RANGE, **f32)
+    self._vr = torch.tensor(cfg.velocity_range, **f32)
+    self._pr = torch.tensor(cfg.pose_range, **f32)
+    self._init_task()
     self._graph = None
     self.reset()
 
@@ -177,6 +302,83 @@ class TrackingFlatEnv:
 
   def _clip(self, name):
     return self.motion[name][self.time_steps]
+
+  # -- task configuration and episode logs ---------------------------------------------------------------------------
+  def _init_task(self) -> None:
+    """The configured terms as both paths use them, and the per-env log state (columns: REWARD_TERMS,
+    TERMINATION_TERMS, METRICS)."""
+    cfg, n = self.cfg, self.num_envs
+    f32 = dict(dtype=torch.float32, device=self.device)
+    rc, tc = cfg.rewards, cfg.terminations
+    self.task_cfg = not cfg.is_base_task()  # the fused kernels' configured path (B2TrackEnvArgs.task_cfg)
+    self.reward_weights = [float(getattr(rc, t)) for t in REWARD_TERMS]
+    self.reward_stds = [float(getattr(rc, t + "_std")) for t in TRACKING_TERMS]
+    self.term_thresholds = [getattr(tc, t) for t in TERMINATION_TERMS[1:]]
+    self._push_r = None if cfg.push_velocity_range is None else torch.tensor(cfg.push_velocity_range, **f32)
+    self.nobs = 5 * self.nu + (15 if cfg.policy_state_estimation else 9)
+    self.episode_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
+    self.finished_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
+    self.term_flags = torch.zeros(n, len(TERMINATION_TERMS), **f32)
+    self.motion_metrics = torch.zeros(n, len(METRICS), **f32)
+    self.finished_metrics = torch.zeros(n, len(METRICS), **f32)
+
+  def _ended(self):
+    """[n, 1] envs whose episode ended in the last step (terminated | truncated, the reference's reset_buf; clip
+    restarts are internal to the command) and their count."""
+    ended = (self.term_flags != 0).any(dim=1, keepdim=True)
+    return ended, ended.sum()
+
+  def _need_logs(self) -> None:
+    if not self.cfg.episode_logs:
+      raise RuntimeError("episode logs are off: build the env with TrackingEnvCfg(episode_logs=True)")
+
+  def reward_log(self) -> dict:
+    """``Episode_Reward/<term>`` of RewardManager.reset (managers/reward_manager.py:61-75) for the envs whose episode
+    ended in the last step: the mean of their episode sums over episode_length_s (NaN when none ended), for all nine
+    terms.  Device tensors, no host synchronisation."""
+    self._need_logs()
+    ended, k = self._ended()
+    mean = torch.where(ended, self.finished_sums, 0.0).sum(0) / k / self.cfg.episode_length_s
+    return {f"Episode_Reward/{t}": mean[i] for i, t in enumerate(REWARD_TERMS)}
+
+  def termination_log(self) -> dict:
+    """``Episode_Termination/<term>`` of TerminationManager.reset (managers/termination_manager.py:73-85): how many of
+    the envs whose episode ended in the last step that term fired for (NaN when none ended); a removed term has no
+    key.  Device tensors, no host synchronisation."""
+    self._need_logs()
+    ended, k = self._ended()
+    count = torch.count_nonzero(self.term_flags, dim=0).float()
+    count = torch.where(k > 0, count, math.nan)
+    on = [True] + [t is not None for t in self.term_thresholds]
+    return {f"Episode_Termination/{t}": count[i] for i, t in enumerate(TERMINATION_TERMS) if on[i]}
+
+  def command_log(self) -> dict:
+    """``Metrics/motion/<error>`` of CommandManager.reset (managers/command_manager.py:128-134, the errors of
+    MotionCommand._update_metrics, tasks/tracking/mdp/commands.py:221-255) for the envs whose episode ended in the last
+    step: the mean of the errors of their last command update (NaN when none ended); with the adaptive sampler also
+    ``sampling_entropy`` / ``sampling_top1_prob`` / ``sampling_top1_bin``.  Device tensors, no host synchronisation."""
+    self._need_logs()
+    ended, k = self._ended()
+    mean = torch.where(ended, self.finished_metrics, 0.0).sum(0) / k
+    out = {f"Metrics/motion/{t}": mean[i] for i, t in enumerate(METRICS)}
+    if self.start_mode == native.START_ADAPTIVE:
+      for i, t in enumerate(("sampling_entropy", "sampling_top1_prob", "sampling_top1_bin")):
+        out[f"Metrics/motion/{t}"] = self._metrics[i]
+    return out
+
+  def _motion_errors(self, frame, pos, quat, lin, ang):
+    """[n, 10] MotionCommand._update_metrics (commands.py:221-255) at clip frames `frame` against the robot's tracked
+    bodies and joints and the current relative targets."""
+    d, a = self.sim.data, self.anchor
+    clip = {k: v[frame] for k, v in self.motion.items()}
+    a_pos = clip["body_pos_w"][:, a] + self.env_origins
+    return torch.stack([
+      (a_pos - pos[:, a]).norm(dim=-1), quat_error_magnitude(clip["body_quat_w"][:, a], quat[:, a]),
+      (clip["body_lin_vel_w"][:, a] - lin[:, a]).norm(dim=-1), (clip["body_ang_vel_w"][:, a] - ang[:, a]).norm(dim=-1),
+      (self.body_pos_relative_w - pos).norm(dim=-1).mean(-1),
+      quat_error_magnitude(self.body_quat_relative_w, quat).mean(-1),
+      (clip["body_lin_vel_w"] - lin).norm(dim=-1).mean(-1), (clip["body_ang_vel_w"] - ang).norm(dim=-1).mean(-1),
+      (clip["joint_pos"] - d.qpos[:, 7:]).norm(dim=-1), (clip["joint_vel"] - d.qvel[:, 6:]).norm(dim=-1)], dim=1)
 
   # -- adaptive start-frame sampler (commands.py:99-110, 256-297, 394-398) -------------------------------
   def _sampler_setup(self) -> None:
@@ -295,12 +497,13 @@ class TrackingFlatEnv:
     jp, jv = d.qpos[:, 7:] - self.default_joint_pos, d.qvel[:, 6:]
     terms = [command, anchor_pos_b, anchor_ori_b, base_lin, base_ang, jp, jv, self.last_action]
     amp = (0.0, 0.25, 0.05, 0.5, 0.2, 0.01, 0.5, 0.0)
+    # each noised term has its own columns of Z, drawn whether or not the term is in the policy group
+    se, noise_on = self.cfg.policy_state_estimation, self.cfg.policy_corruption
     noisy, k = [], 0
-    for t, a in zip(terms, amp):
-      if a == 0.0:
-        noisy.append(t)
-      else:
-        noisy.append(t + (Z[:, k:k + t.shape[1]] * 2 - 1) * a)
+    for i, (t, a) in enumerate(zip(terms, amp)):
+      if se or i not in (1, 3):  # without state estimation: no motion_anchor_pos_b, no base_lin_vel
+        noisy.append(t if a == 0.0 or not noise_on else t + (Z[:, k:k + t.shape[1]] * 2 - 1) * a)
+      if a != 0.0:
         k += t.shape[1]
     rq = r_quat[:, None, :].expand(-1, len(BODY_NAMES), -1)
     body_pos_b = quat_apply_inverse(rq, pos - r_pos[:, None, :]).flatten(1)
@@ -310,6 +513,8 @@ class TrackingFlatEnv:
 
   # -- API -----------------------------------------------------------------------------------------
   def reset(self):
+    for t in (self.episode_sums, self.term_flags, self.motion_metrics):  # the logs start over
+      t.zero_()
     all_ = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
     self._resample(all_, all_, self._rand(self.num_envs, 13 + self.nu))
     self.sim.forward()
@@ -355,7 +560,7 @@ class TrackingFlatEnv:
     self._reward = torch.zeros(n, **f32)
     self._term = torch.zeros(n, dtype=torch.bool, device=dev)
     self._trunc = torch.zeros(n, dtype=torch.bool, device=dev)
-    self._obs = torch.zeros(n, 5 * nu + 15, **f32)
+    self._obs = torch.zeros(n, self.nobs, **f32)
     self._critic = torch.zeros(n, 5 * nu + 15 + 9 * nb, **f32)
     self._body_idx32 = self.robot.indexing.body_ids[self.body_idx].to(torch.int32).contiguous()
     self._ee_idx32 = self.ee_idx.to(torch.int32).contiguous()
@@ -377,8 +582,8 @@ class TrackingFlatEnv:
       assert t.is_contiguous(), k
       setattr(A, k, t.data_ptr())
     for k in range(6):
-      A.pose_range[2 * k], A.pose_range[2 * k + 1] = POSE_RANGE[k]
-      A.vel_range[2 * k], A.vel_range[2 * k + 1] = VELOCITY_RANGE[k]
+      A.pose_range[2 * k], A.pose_range[2 * k + 1] = self.cfg.pose_range[k]
+      A.vel_range[2 * k], A.vel_range[2 * k + 1] = self.cfg.velocity_range[k]
     A.step_dt = self.step_dt
     A.jp_lo, A.jp_hi = self.cfg.joint_position_range
     A.push_lo, A.push_hi = self.cfg.push_interval_s
@@ -396,6 +601,23 @@ class TrackingFlatEnv:
       ptr.update(sampler)
       A.adaptive_alpha, A.adaptive_uniform_ratio = self.cfg.adaptive_alpha, self.cfg.adaptive_uniform_ratio
       A.nbins, A.adaptive_kernel_size = self.bin_count, self.cfg.adaptive_kernel_size
+    if self.task_cfg:
+      logs = dict(episode_sums=self.episode_sums, finished_sums=self.finished_sums, term_flags=self.term_flags,
+                  motion_metrics=self.motion_metrics, finished_metrics=self.finished_metrics)
+      for k, t in logs.items():
+        assert t.is_contiguous() and t.dtype == torch.float32, k
+        setattr(A, k, t.data_ptr())
+      ptr.update(logs)
+      A.task_cfg = 1
+      A.weight[:] = self.reward_weights
+      A.std2[:] = [s**2 for s in self.reward_stds]  # (the fp32 value of the double the torch path divides by)
+      for k, v in enumerate(self.term_thresholds):
+        A.term_on[k], A.term_threshold[k] = v is not None, 0.0 if v is None else v
+      if self.cfg.push_velocity_range is not None:
+        A.push_on = 1
+        for k in range(6):
+          A.push_range[2 * k], A.push_range[2 * k + 1] = self.cfg.push_velocity_range[k]
+      A.policy_state_estimation, A.policy_corruption = self.cfg.policy_state_estimation, self.cfg.policy_corruption
     self._native_args = A
     self._keep = ptr
 
@@ -450,33 +672,59 @@ class TrackingFlatEnv:
     a_pos = self._clip("body_pos_w")[:, self.anchor] + self.env_origins
     a_quat = self._clip("body_quat_w")[:, self.anchor]
     r_pos, r_quat = pos[:, self.anchor], quat[:, self.anchor]
-    # terminations (tracking_env_cfg.py:253-278)
+    # terminations (tracking_env_cfg.py:253-278); a removed term never fires
     truncated = self.episode_length_buf >= self.max_episode_length
-    bad_z = (a_pos[:, 2] - r_pos[:, 2]).abs() > 0.25
+    th, never = self.term_thresholds, torch.zeros_like(truncated)
+    bad_z = (a_pos[:, 2] - r_pos[:, 2]).abs() > th[0] if th[0] is not None else never
     g = self.robot.gravity_vec_w
-    bad_ori = (quat_apply_inverse(a_quat, g)[:, 2] - quat_apply_inverse(r_quat, g)[:, 2]).abs() > 0.8
+    bad_ori = ((quat_apply_inverse(a_quat, g)[:, 2] - quat_apply_inverse(r_quat, g)[:, 2]).abs() > th[1]
+               if th[1] is not None else never)
     ee_err = (self.body_pos_relative_w[:, self.ee_idx, 2] - pos[:, self.ee_idx, 2]).abs()
-    terminated = bad_z | bad_ori | (ee_err > 0.25).any(dim=1)
+    bad_ee = (ee_err > th[2]).any(dim=1) if th[2] is not None else never
+    terminated = bad_z | bad_ori | bad_ee
     if self.start_mode == native.START_ADAPTIVE:  # failures, in the bin of the frame reached (commands.py:257-265)
       fail_bin = (self.time_steps * self.bin_count // self.T).clamp_(0, self.bin_count - 1)
       self._bin_failed_cur.index_add_(0, fail_bin, terminated.float())
-    # rewards (:200-250)
-    r = 0.5 * torch.exp(-((a_pos - r_pos) ** 2).sum(-1) / 0.3**2)
-    r = r + 0.5 * torch.exp(-quat_error_magnitude(a_quat, r_quat) ** 2 / 0.4**2)
-    r = r + torch.exp(-((self.body_pos_relative_w - pos) ** 2).sum(-1).mean(-1) / 0.3**2)
-    r = r + torch.exp(-(quat_error_magnitude(self.body_quat_relative_w, quat) ** 2).mean(-1) / 0.4**2)
-    r = r + torch.exp(-((self._clip("body_lin_vel_w") - lin) ** 2).sum(-1).mean(-1) / 1.0**2)
-    r = r + torch.exp(-((self._clip("body_ang_vel_w") - ang) ** 2).sum(-1).mean(-1) / 3.14**2)
-    r = r - 0.1 * ((action - self.last_action) ** 2).sum(1)
+    # rewards (:200-250): each term times its weight; a term at weight 0 is not evaluated
+    W, sd = self.reward_weights, self.reward_stds
     jp, lim = d.qpos[:, 7:], self.robot.soft_joint_pos_limits
-    r = r - 10.0 * ((lim[..., 0] - jp).clamp(min=0) + (jp - lim[..., 1]).clamp(min=0)).sum(1)
-    r = r - 10.0 * d.sensordata[:, self.self_collision_adr[0]]
-    reward = r * self.step_dt
+    terms = (
+      lambda: torch.exp(-((a_pos - r_pos) ** 2).sum(-1) / sd[0]**2),
+      lambda: torch.exp(-quat_error_magnitude(a_quat, r_quat) ** 2 / sd[1]**2),
+      lambda: torch.exp(-((self.body_pos_relative_w - pos) ** 2).sum(-1).mean(-1) / sd[2]**2),
+      lambda: torch.exp(-(quat_error_magnitude(self.body_quat_relative_w, quat) ** 2).mean(-1) / sd[3]**2),
+      lambda: torch.exp(-((self._clip("body_lin_vel_w") - lin) ** 2).sum(-1).mean(-1) / sd[4]**2),
+      lambda: torch.exp(-((self._clip("body_ang_vel_w") - ang) ** 2).sum(-1).mean(-1) / sd[5]**2),
+      lambda: ((action - self.last_action) ** 2).sum(1),
+      lambda: ((lim[..., 0] - jp).clamp(min=0) + (jp - lim[..., 1]).clamp(min=0)).sum(1),
+      lambda: d.sensordata[:, self.self_collision_adr[0]])
+    zero = torch.zeros(n, device=self.device)
+    vals = [W[i] * f() if W[i] != 0.0 else zero for i, f in enumerate(terms)]
+    r = None
+    for i, v in enumerate(vals):
+      if W[i] != 0.0:
+        r = v if r is None else r + v
+    reward = (zero if r is None else r) * self.step_dt
     self.last_action.copy_(action)
     done = terminated | truncated
     self.log_row.copy_(torch.stack([reward, terminated.float(), truncated.float()], dim=1))
+    # episode logs (RewardManager / TerminationManager), kept where the fused kernels keep them (task_cfg): a done
+    # env's sums end their episode
+    dk = done.unsqueeze(1)
+    if self.task_cfg:
+      sums = self.episode_sums + torch.stack(vals, dim=1) * self.step_dt
+      self.finished_sums.copy_(torch.where(dk, sums, self.finished_sums))
+      self.episode_sums.copy_(torch.where(dk, 0.0, sums))
+      self.term_flags.copy_(torch.stack([truncated, bad_z, bad_ori, bad_ee], dim=1).float())
+      # motion errors (MotionCommand._update_metrics): a done env hands over those of the last update; every other
+      # env takes them now, at its frame before the clip steps (a done env takes its own after the forward, below)
+      self.finished_metrics.copy_(torch.where(dk, self.motion_metrics, self.finished_metrics))
+      e = self._motion_errors(self.time_steps, pos, quat, lin, ang)
+      self.motion_metrics.copy_(torch.where(dk, self.motion_metrics, e))
     # reset onto the clip (RSI); then the clip's time step: envs that ran off its end restart on it.  Both rewrite
-    # the whole state of their envs, so one forward over the union follows (the reference runs one per event)
+    # the whole state of their envs, so one forward over the union follows (the reference runs one per event).  An
+    # env reset onto the clip's last frame is restarted in the same step, so its state is written twice before that
+    # forward and the motion errors it takes after it see the second state (the reference sees the first)
     self._resample(done, done, U[:, 0:S])
     self.episode_length_buf.copy_(torch.where(done, torch.zeros_like(self.episode_length_buf), self.episode_length_buf))
     self.last_action.copy_(torch.where(done.unsqueeze(1), torch.zeros_like(self.last_action), self.last_action))
@@ -487,16 +735,22 @@ class TrackingFlatEnv:
       self._sampler_step()
     self._done_buf.copy_(done | ended)
     self.sim.forward(env_mask=self._done_buf)
+    # a done env's motion errors: its reset state against the frame before the clip stepped and the stale targets
+    if self.task_cfg:
+      e = self._motion_errors((self.time_steps - 1).clamp(min=0), *self._robot_bodies())
+      self.motion_metrics.copy_(torch.where(dk, e, self.motion_metrics))
     self._update_command()
-    # interval push (push_by_setting_velocity with VELOCITY_RANGE, tracking_env_cfg.py:155-161)
-    self.push_time_left -= self.step_dt
-    push = self.push_time_left <= 0
-    P = U[:, 2 * S:2 * S + 7]
-    vel_w = self.robot.root_link_vel_w + P[:, 0:6] * (self._vr[:, 1] - self._vr[:, 0]) + self._vr[:, 0]
-    vel = torch.cat([vel_w[:, 0:3], quat_apply_inverse(self.robot.root_link_quat_w, vel_w[:, 3:6])], dim=1)
-    d.qvel[:, 0:6] = torch.where(push.unsqueeze(1), vel, d.qvel[:, 0:6])
-    lo_t, hi_t = cfg.push_interval_s
-    self.push_time_left.copy_(torch.where(push, P[:, 6] * (hi_t - lo_t) + lo_t, self.push_time_left))
+    # interval push (push_by_setting_velocity, tracking_env_cfg.py:155-161); none without a push range
+    if self._push_r is not None:
+      pr = self._push_r
+      self.push_time_left -= self.step_dt
+      push = self.push_time_left <= 0
+      P = U[:, 2 * S:2 * S + 7]
+      vel_w = self.robot.root_link_vel_w + P[:, 0:6] * (pr[:, 1] - pr[:, 0]) + pr[:, 0]
+      vel = torch.cat([vel_w[:, 0:3], quat_apply_inverse(self.robot.root_link_quat_w, vel_w[:, 3:6])], dim=1)
+      d.qvel[:, 0:6] = torch.where(push.unsqueeze(1), vel, d.qvel[:, 0:6])
+      lo_t, hi_t = cfg.push_interval_s
+      self.push_time_left.copy_(torch.where(push, P[:, 6] * (hi_t - lo_t) + lo_t, self.push_time_left))
     policy, critic = self.observations(U[:, 2 * S + 7:])
     return policy, reward, terminated, truncated, self._extras(critic)
 

@@ -404,6 +404,15 @@ class VelocityFlatEnv:
     return {f"Episode_Reward/{t}": mean[i] for i, t in enumerate(REWARD_TERMS)
             if i < NFIXED or self.reward_weights[i - NFIXED] != 0.0}
 
+  def termination_log(self) -> dict:
+    """``Episode_Termination/time_out`` and ``fell_over`` of TerminationManager.reset
+    (managers/termination_manager.py:73-85): how many of the envs whose episode ended in the last step that term fired
+    for (NaN when none ended).  Device tensors, no host synchronisation."""
+    done = self._done_buf
+    flags = torch.stack([self.log_row[:, 2], self.log_row[:, 1]], dim=1)  # (truncated, terminated) of the last step
+    count = torch.where(done.any(), torch.count_nonzero(flags, dim=0).float(), math.nan)
+    return {"Episode_Termination/time_out": count[0], "Episode_Termination/fell_over": count[1]}
+
   def _init_native(self) -> None:
     from mjlab_b200.sim import native
 

@@ -93,7 +93,15 @@ class B2TrackEnvArgs(ctypes.Structure):
     + [(n, ctypes.c_void_p) for n in ("adaptive_kernel", "cdf", "bin_fail_ema", "bin_fail_cur", "metrics")]
     + [(n, ctypes.c_float) for n in ("adaptive_alpha", "adaptive_uniform_ratio")]
     + [(n, ctypes.c_int32) for n in ("nbins", "adaptive", "adaptive_kernel_size")]
+    + [("task_cfg", ctypes.c_int32), ("weight", ctypes.c_float * 9), ("std2", ctypes.c_float * 6),
+       ("term_threshold", ctypes.c_float * 3), ("term_on", ctypes.c_int32 * 3), ("push_range", ctypes.c_float * 12)]
+    + [(n, ctypes.c_int32) for n in ("push_on", "policy_state_estimation", "policy_corruption")]
+    + [(n, ctypes.c_void_p) for n in ("episode_sums", "finished_sums", "term_flags", "motion_metrics",
+                                      "finished_metrics")]
   )
+
+
+TRACKENV_NREW, TRACKENV_NTERM, TRACKENV_NMETRIC = 9, 4, 10  # B2_TRACKENV_N*: log columns of B2TrackEnvArgs
 
 
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
