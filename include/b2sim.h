@@ -113,7 +113,7 @@ int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_ho
  * ManagerBasedRlEnv.step (manager_based_rl_env.py:106-147) does before and after the decimation loop for
  * tasks/velocity/velocity_env_cfg.py, as two launches. All pointers are device pointers. */
 #define B2_VELENV_NU(nu) (16 + 9 + 2 * (nu))
-#define B2_VELENV_NTERM 14 /* reward terms with an episode sum (B2VelEnvArgs.rewards) */
+#define B2_VELENV_NTERM 14 /* reward terms with an episode sum (B2VelEnvArgs.episode_sums) */
 #define B2_VELENV_NSTAGE 8 /* stages of the command-velocity curriculum (B2VelEnvArgs.n_stage) */
 typedef struct B2VelEnvArgs {
   const float* action;            /* [n][nu] */
@@ -154,8 +154,8 @@ typedef struct B2VelEnvArgs {
   float move_up_dist, episode_length_s;
   int32_t rows, cols, curriculum;
   /* opt-in reward terms of the reference's velocity task (tasks/velocity/mdp/rewards.py:52-190) and shared penalties
-   * (envs/mdp/rewards.py:22-127), with per-term episode sums (managers/reward_manager.py:61-89); rewards = 0 leaves
-   * every field below unread.  Terms, in the order of the episode-sum columns (B2_VELENV_NTERM):
+   * (envs/mdp/rewards.py:22-127), with per-term episode sums (managers/reward_manager.py:61-89).  Terms, in the order
+   * of the episode-sum columns (B2_VELENV_NTERM):
    *   0-4 the fixed terms: track_lin_vel_exp, track_ang_vel_exp, pose, dof_pos_limits, action_rate_l2 (weights 1, 1,
    *       1, -1, -0.1, not configurable);
    *   5 air_time, 6 feet_slide, 7 foot_clearance, 8 is_alive, 9 is_terminated, 10 joint_torques_l2, 11 joint_acc_l2,
@@ -164,7 +164,7 @@ typedef struct B2VelEnvArgs {
    * w_i r_i) step_dt.  A foot is in contact when sensordata[adr] > 0; a geom's linear velocity is
    * cvel[3:6] - cvel[0:3] x (subtree_com[root_body] - geom_xpos).  Per-foot state of a done env is zeroed after its
    * reward.  episode_sums[w][i] += w_i r_i step_dt for all 14 terms; a done env's row is copied to finished_sums and
-   * zeroed.  A null episode_sums skips both. */
+   * zeroed. */
   float weight[B2_VELENV_NTERM - 5]; /* of terms 5-13 */
   float air_threshold_min, air_threshold_max, air_command_threshold, air_command_scale_width;
   float clearance_target_height, clearance_std, clearance_tanh_mult;
@@ -181,36 +181,33 @@ typedef struct B2VelEnvArgs {
   float* air_time;                /* [n][n_air] in/out: current air time */
   float* contact_time;            /* [n][n_air] in/out: current contact time */
   float* last_air_time;           /* [n][n_air] in/out: air time of the last landing */
-  float* episode_sums;            /* [n][B2_VELENV_NTERM] in/out, or null */
+  float* episode_sums;            /* [n][B2_VELENV_NTERM] in/out */
   float* finished_sums;           /* [n][B2_VELENV_NTERM] out: the sums of the episode a done env just ended */
-  int32_t rewards;
   /* the command term as the reference's tasks configure it (UniformVelocityCommandCfg,
    * tasks/velocity/mdp/velocity_command.py:179-203), the command-velocity curriculum (commands_vel,
    * tasks/velocity/mdp/curriculums.py:55-74), per-joint posture widths (posture, envs/mdp/rewards.py:73-104) and the
-   * command's metrics (velocity_command.py:43-62).  Each part is off when its fields are zero or null:
-   *   command = 0: the ranges x +-1, y +-0.5, yaw +-1, heading +-pi, stiffness 0.5, 10 % standing, timer 3..8 s
-   *     (b2_velenv_post writes them into the fields below).  A component is drawn as mid + (2u - 1) half (one IEEE
-   *     product and one IEEE sum), the timer as resample_lo + resample_span u, standing as u <= rel_standing; the
-   *     heading command is clamp(heading_stiffness wrap(target - heading), ang_lo, ang_hi).
+   * command's metrics (velocity_command.py:43-62):
+   *   A component is drawn as mid + (2u - 1) half (one IEEE product and one IEEE sum), the timer as resample_lo +
+   *   resample_span u (resample_lo > 0), standing as u <= rel_standing; the heading command is
+   *   clamp(heading_stiffness wrap(target - heading), ang_lo, ang_hi).
    *   n_stage > 0: counter = *step_counter + 1 is the step's common_step_counter; the lin_vel_x and ang_vel_z ranges
    *     of the step are those of the last stage s in list order with stage_step[s] < counter (the cfg's when none
    *     is).  b2_velenv_post advances *step_counter after the post kernel (one one-thread launch).
-   *   posture_inv_std2: the pose term is exp(-mean_j(d_j^2 / std_j^2)); null: exp(-mean_j(d_j^2) / 0.09).
-   *   metric_xy: every env adds |cmd_xy - v_b,xy| / metric_steps and |cmd_z - w_b,z| / metric_steps, from the command
-   *     before this step's timer resample and the post-physics velocity.  A done env first moves its sums to
-   *     finished_metrics and restarts them at 0; its first increment uses the fresh draw (before heading control and
-   *     standing) and the post-reset state.  Null skips the metrics. */
+   *   The pose term is exp(-mean_j(d_j^2 posture_inv_std2[j])).
+   *   Every env adds |cmd_xy - v_b,xy| / metric_steps and |cmd_z - w_b,z| / metric_steps to metric_xy / metric_yaw,
+   *     from the command before this step's timer resample and the post-physics velocity.  A done env first moves its
+   *     sums to finished_metrics and restarts them at 0; its first increment uses the fresh draw (before heading
+   *     control and standing) and the post-reset state. */
   float cmd_mid[4], cmd_half[4];  /* lin_vel_x, lin_vel_y, ang_vel_z, heading: (lo + hi) / 2, (hi - lo) / 2 */
   float ang_lo, ang_hi;           /* ang_vel_z range */
   float heading_stiffness, rel_standing, resample_lo, resample_span;
-  int32_t command_cfg;
   int32_t n_stage;                /* <= B2_VELENV_NSTAGE */
   int32_t stage_step[B2_VELENV_NSTAGE];
   float stage_mid[B2_VELENV_NSTAGE], stage_half[B2_VELENV_NSTAGE]; /* of the stage's range, as cmd_mid / cmd_half */
   float stage_lo[B2_VELENV_NSTAGE], stage_hi[B2_VELENV_NSTAGE];
   int32_t* step_counter;          /* [1] in/out: common_step_counter */
-  const float* posture_inv_std2;  /* [nu] 1 / std^2 per joint, or null */
-  float* metric_xy;               /* [n] in/out: error_vel_xy of the running command episode, or null */
+  const float* posture_inv_std2;  /* [nu] 1 / std^2 per joint */
+  float* metric_xy;               /* [n] in/out: error_vel_xy of the running command episode */
   float* metric_yaw;              /* [n] in/out: error_vel_yaw */
   float* finished_metrics;        /* [n][2] out: (xy, yaw) of the episode a done env just ended */
   float metric_steps;             /* resampling_time_range[1] / step_dt */
@@ -274,25 +271,24 @@ typedef struct B2TrackEnvArgs {
   float adaptive_alpha, adaptive_uniform_ratio;
   int32_t nbins, adaptive, adaptive_kernel_size;
   /* the task as a cfg class configures it (tracking_env_cfg.py:88-278, tasks/tracking/config/g1/flat_env_cfg.py) and
-   * the episode logs of its managers; task_cfg = 0 leaves every field below unread and runs the base task's literal
-   * terms (weights 0.5 0.5 1 1 1 1 -0.1 -10 -10, stds 0.3 0.4 0.3 0.4 1 3.14, thresholds 0.25 0.8 0.25, push from
-   * vel_range, both observation switches on) with no logs.  The RSI ranges are pose_range / vel_range above.
+   * the episode logs of its managers.  The RSI ranges are pose_range / vel_range above.
    * Reward terms, in the order of the episode-sum columns (B2_TRACKENV_NREW): 0 motion_global_root_pos,
    * 1 motion_global_root_ori, 2 motion_body_pos, 3 motion_body_ori, 4 motion_body_lin_vel, 5 motion_body_ang_vel
    * (exp(-err / std2[i])), 6 action_rate_l2, 7 joint_limit, 8 self_collisions.  A term at weight 0 is not evaluated.
-   * reward = (sum of w_i r_i) step_dt; episode_sums[w][i] += w_i r_i step_dt.
+   * reward = (sum of w_i r_i) step_dt.
    * Terminations, in the order of term_flags (B2_TRACKENV_NTERM): 0 time_out, 1 anchor_pos, 2 anchor_ori,
-   * 3 ee_body_pos; term_on[k] = 0 removes term k + 1.  term_flags[w] holds every env's flags of this step.
-   * Motion errors (B2_TRACKENV_NMETRIC, commands.py:221-255): 0 anchor_pos, 1 anchor_rot, 2 anchor_lin_vel,
-   * 3 anchor_ang_vel, 4 body_pos, 5 body_rot, 6 body_lin_vel, 7 body_ang_vel (means of norms over the tracked bodies),
-   * 8 joint_pos, 9 joint_vel (norms over the joints).  An env that is not done takes them in post1 at its frame
-   * before the clip steps; a done env in post2, after the forward, at frame max(time_steps - 1, 0) against the
-   * relative targets of the previous post2.  A done env's episode_sums and motion_metrics rows move to finished_sums /
-   * finished_metrics in post1 (the episode sums restart at 0).
+   * 3 ee_body_pos; term_on[k] = 0 removes term k + 1.
    * policy_state_estimation = 0 drops motion_anchor_pos_b and base_lin_vel from the policy row ([n][5 nu + 9]); their
    * noise columns of U are still drawn.  policy_corruption = 0 writes the policy terms without noise.  push_on = 0:
-   * no push, push_time_left untouched. */
-  int32_t task_cfg;
+   * no push, push_time_left untouched.
+   * The episode logs are the five arrays at the end, all set or all null (no logs).  episode_sums[w][i] +=
+   * w_i r_i step_dt; term_flags[w] holds every env's flags of this step.  Motion errors (B2_TRACKENV_NMETRIC,
+   * commands.py:221-255): 0 anchor_pos, 1 anchor_rot, 2 anchor_lin_vel, 3 anchor_ang_vel, 4 body_pos, 5 body_rot,
+   * 6 body_lin_vel, 7 body_ang_vel (means of norms over the tracked bodies), 8 joint_pos, 9 joint_vel (norms over the
+   * joints).  An env that is not done takes them in post1 at its frame before the clip steps; a done env in post2,
+   * after the forward, at frame max(time_steps - 1, 0) against the relative targets of the previous post2.  A done
+   * env's episode_sums and motion_metrics rows move to finished_sums / finished_metrics in post1 (the episode sums
+   * restart at 0). */
   float weight[9], std2[6];       /* B2_TRACKENV_NREW weights; std^2 of reward terms 0-5 */
   float term_threshold[3];        /* anchor_pos, anchor_ori, ee_body_pos */
   int32_t term_on[3];

@@ -3,7 +3,7 @@
 // with the terms of tasks/velocity/velocity_env_cfg.py) as two kernels instead of ~90 tiny torch launches:
 //   pre  : ctrl = default_joint_pos + action_scale * action                     (joint_actions.py:85-103)
 //   post : episode counter, terminations (bad_orientation, time_out), rewards (the five fixed terms, the opt-in terms
-//          of B2VelEnvArgs.rewards and their episode sums), the terrain-level curriculum of
+//          of B2VelEnvArgs.weight and their episode sums), the terrain-level curriculum of
 //          the reset envs (opt-in, curriculums.py:18-52), masked reset (events.py:43-124), interval push
 //          (events.py:127-143), command resample (configurable ranges, the opt-in command-velocity curriculum and
 //          the command's metrics), observations.
@@ -149,75 +149,69 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   b2e_rot_inv(q, lin, lb);
   float e0 = c0 - lb[0], e1 = c1 - lb[1], e2 = c2 - wz;
   float r_lin = expf(-(e0 * e0 + e1 * e1) / 0.25f), r_ang = expf(-(e2 * e2) / 0.25f);
-  float pose = 0.f, wpose = 0.f, lim = 0.f, rate = 0.f;
-  const float* inv_std2 = A.posture_inv_std2;  // per-joint widths: wpose; the single width keeps its own sum
+  float pose = 0.f, lim = 0.f, rate = 0.f;
   for (int a = lane; a < nu; a += 32) {
     float jp = qpos[7 + a], dj = jp - A.default_joint_pos[a];
-    pose += dj * dj;
-    if (inv_std2) wpose += dj * dj * inv_std2[a];
+    pose += dj * dj * A.posture_inv_std2[a];
     lim += fmaxf(A.soft_lo[a] - jp, 0.f) + fmaxf(jp - A.soft_hi[a], 0.f);
     float da = act[a] - last[a];
     rate += da * da;
   }
-  pose = b2e_wsum(inv_std2 ? wpose : pose); lim = b2e_wsum(lim); rate = b2e_wsum(rate);
+  pose = b2e_wsum(pose); lim = b2e_wsum(lim); rate = b2e_wsum(rate);
   bool done = term || trunc;
-  // opt-in terms (B2VelEnvArgs.rewards): r[i] is term 5 + i unweighted, evaluated only at a non-zero weight
+  // opt-in terms: r[i] is term 5 + i unweighted, evaluated only at a non-zero weight
   float r[B2_VELENV_NTERM - 5] = {}, extra = 0.f;
-  bool any = false;
-  if (A.rewards) {
-    const float* W = A.weight;
-    const float* sd = dd.sensordata.p + (size_t)w * dd.sensordata.stride;
-    if (W[0] != 0.f) {  // air_time, scaled by the command (smooth or hard)
-      const float cn = b2e_norm2_rn(c0, c1);
-      const float s = A.air_hard_scale ? (cn > A.air_command_threshold ? 1.f : 0.f)
-                                       : 0.5f * (1.f + tanhf((cn - A.air_command_threshold) / A.air_command_scale_width));
-      r[0] = b2e_air_time(A, sd, w, lane, done) * s;
+  const float* W = A.weight;
+  const float* sd = dd.sensordata.p + (size_t)w * dd.sensordata.stride;
+  if (W[0] != 0.f) {  // air_time, scaled by the command (smooth or hard)
+    const float cn = b2e_norm2_rn(c0, c1);
+    const float s = A.air_hard_scale ? (cn > A.air_command_threshold ? 1.f : 0.f)
+                                     : 0.5f * (1.f + tanhf((cn - A.air_command_threshold) / A.air_command_scale_width));
+    r[0] = b2e_air_time(A, sd, w, lane, done) * s;
+  }
+  if (W[1] != 0.f) {  // feet_slide
+    float v = 0.f;
+    if (lane < A.n_slide && sd[A.slide_sensor_adr[lane]] > 0.f) {
+      float vx, vy, z;
+      b2e_geom_vel(dd, w, A.slide_geom[lane], A.slide_body[lane], A.root_body, vx, vy, z);
+      v = sqrtf(vx * vx + vy * vy);
     }
-    if (W[1] != 0.f) {  // feet_slide
-      float v = 0.f;
-      if (lane < A.n_slide && sd[A.slide_sensor_adr[lane]] > 0.f) {
-        float vx, vy, z;
-        b2e_geom_vel(dd, w, A.slide_geom[lane], A.slide_body[lane], A.root_body, vx, vy, z);
-        v = sqrtf(vx * vx + vy * vy);
-      }
-      r[1] = b2e_wsum(v);
+    r[1] = b2e_wsum(v);
+  }
+  if (W[2] != 0.f) {  // foot_clearance_reward
+    float v = 0.f;
+    if (lane < A.n_clear) {
+      float vx, vy, z;
+      b2e_geom_vel(dd, w, A.clear_geom[lane], A.clear_body[lane], A.root_body, vx, vy, z);
+      const float e = z - A.clearance_target_height;
+      v = e * e * tanhf(A.clearance_tanh_mult * sqrtf(vx * vx + vy * vy));
     }
-    if (W[2] != 0.f) {  // foot_clearance_reward
-      float v = 0.f;
-      if (lane < A.n_clear) {
-        float vx, vy, z;
-        b2e_geom_vel(dd, w, A.clear_geom[lane], A.clear_body[lane], A.root_body, vx, vy, z);
-        const float e = z - A.clearance_target_height;
-        v = e * e * tanhf(A.clearance_tanh_mult * sqrtf(vx * vx + vy * vy));
-      }
-      r[2] = expf(-b2e_wsum(v) / A.clearance_std);
+    r[2] = expf(-b2e_wsum(v) / A.clearance_std);
+  }
+  r[3] = term ? 0.f : 1.f;  // is_alive
+  r[4] = term ? 1.f : 0.f;  // is_terminated
+  if (W[5] != 0.f || W[6] != 0.f || W[7] != 0.f) {  // joint_torques_l2, joint_acc_l2, electrical_power_cost
+    const float* af = dd.actuator_force.p + (size_t)w * dd.actuator_force.stride;
+    const float* qa = dd.qacc.p + (size_t)w * dd.qacc.stride;
+    float tau = 0.f, acc = 0.f, pw = 0.f;
+    for (int a = lane; a < nu; a += 32) {
+      const float f = af[a], j = qa[6 + a];
+      tau += f * f;
+      acc += j * j;
+      pw += fmaxf(f * qvel[6 + a], 0.f);
     }
-    r[3] = term ? 0.f : 1.f;  // is_alive
-    r[4] = term ? 1.f : 0.f;  // is_terminated
-    if (W[5] != 0.f || W[6] != 0.f || W[7] != 0.f) {  // joint_torques_l2, joint_acc_l2, electrical_power_cost
-      const float* af = dd.actuator_force.p + (size_t)w * dd.actuator_force.stride;
-      const float* qa = dd.qacc.p + (size_t)w * dd.qacc.stride;
-      float tau = 0.f, acc = 0.f, pw = 0.f;
-      for (int a = lane; a < nu; a += 32) {
-        const float f = af[a], j = qa[6 + a];
-        tau += f * f;
-        acc += j * j;
-        pw += fmaxf(f * qvel[6 + a], 0.f);
-      }
-      r[5] = b2e_wsum(tau); r[6] = b2e_wsum(acc); r[7] = b2e_wsum(pw);
-    }
-    r[8] = gb[0] * gb[0] + gb[1] * gb[1];  // flat_orientation_l2
+    r[5] = b2e_wsum(tau); r[6] = b2e_wsum(acc); r[7] = b2e_wsum(pw);
+  }
+  r[8] = gb[0] * gb[0] + gb[1] * gb[1];  // flat_orientation_l2
 #pragma unroll
-    for (int i = 0; i < B2_VELENV_NTERM - 5; i++) {
-      r[i] = W[i] != 0.f ? r[i] * W[i] : 0.f;  // (a term at weight 0 adds nothing, not 0 * its value)
-      any = any || W[i] != 0.f;
-      extra += r[i];
-    }
+  for (int i = 0; i < B2_VELENV_NTERM - 5; i++) {
+    r[i] = W[i] != 0.f ? r[i] * W[i] : 0.f;  // (a term at weight 0 adds nothing, not 0 * its value)
+    extra += r[i];
   }
   __syncwarp();  // every lane holds the pre-reset state it needs; writes may start
-  float r_pose = inv_std2 ? expf(-(pose / (float)nu)) : expf(-(pose / (float)nu) / 0.09f);
+  float r_pose = expf(-(pose / (float)nu));
   const float fixed = r_lin + r_ang + r_pose - lim - 0.1f * rate;
-  const float reward = any ? (fixed + extra) * A.step_dt : fixed * A.step_dt;
+  const float reward = (fixed + extra) * A.step_dt;
   if (lane == 0) {
     A.reward[w] = reward;
     A.terminated[w] = term; A.truncated[w] = trunc; A.done[w] = done;
@@ -225,7 +219,7 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     A.log_row[3 * (size_t)w + 2] = trunc ? 1.f : 0.f;
   }
   // episode sums (RewardManager.compute / reset): column k on lane k
-  if (A.rewards && A.episode_sums && lane < B2_VELENV_NTERM) {
+  if (lane < B2_VELENV_NTERM) {
     float v = lane == 0 ? r_lin : lane == 1 ? r_ang : lane == 2 ? r_pose : lane == 3 ? -lim : lane == 4 ? -0.1f * rate : 0.f;
 #pragma unroll
     for (int i = 0; i < B2_VELENV_NTERM - 5; i++)
@@ -276,7 +270,7 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   {
     // heading_w = atan2 of the body x axis in the world (entity/data.py:480-484), from the post-reset pose
     float qw = qpos[3], qx = qpos[4], qy = qpos[5], qz = qpos[6];
-    if (A.metric_xy && lane == 0) {
+    if (lane == 0) {
       // metrics (CommandTerm.reset, then _update_metrics in compute): a done env hands its sums over and restarts;
       // the increment takes the fresh draw of a done env and every other env's command from before the resample,
       // with the velocity of the post-reset state (before the push)

@@ -140,11 +140,10 @@ __device__ __forceinline__ void motion_errors(const B2TrackEnvArgs& A, int lane,
                                               V3 pos, Q quat, V3 lin, V3 ang, V3 rel_p, Q rel_q, const float* qpos,
                                               const float* qvel, int nu, float* out) {
   const size_t fb = (size_t)fr * A.nb;
+  // the anchor's errors first: its clip and robot poses are not held across the per-body errors
   const V3 cpa = ldv(A.m_body_pos + 3 * (fb + A.anchor));
-  const V3 a_pos = {cpa.x + org.x, cpa.y + org.y, cpa.z + org.z};
-  const Q a_quat = ldq(A.m_body_quat + 4 * (fb + A.anchor));
-  const V3 r_pos = bcastv(pos, A.anchor);
-  const Q r_quat = bcastq(quat, A.anchor);
+  const float anchor_pos = norm3({cpa.x + org.x, cpa.y + org.y, cpa.z + org.z}, bcastv(pos, A.anchor));
+  const float anchor_rot = qerr(ldq(A.m_body_quat + 4 * (fb + A.anchor)), bcastq(quat, A.anchor));
   float ep = 0.f, eq = 0.f, el = 0.f, ea = 0.f;
   if (hasb) {
     ep = norm3(rel_p, pos);
@@ -163,7 +162,7 @@ __device__ __forceinline__ void motion_errors(const B2TrackEnvArgs& A, int lane,
   sj = sqrtf(wsum(sj));
   sv = sqrtf(wsum(sv));
   if (lane == 0) {
-    out[0] = norm3(a_pos, r_pos); out[1] = qerr(a_quat, r_quat); out[2] = anchor_lin; out[3] = anchor_ang;
+    out[0] = anchor_pos; out[1] = anchor_rot; out[2] = anchor_lin; out[3] = anchor_ang;
     out[4] = ep; out[5] = eq; out[6] = el; out[7] = ea; out[8] = sj; out[9] = sv;
   }
 }
@@ -201,6 +200,14 @@ __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackE
   float* last = A.last_action + (size_t)w * nu;
   long long ts = A.time_steps[w];
   int ep = A.episode_length[w] + 1;
+  // the joint terms' sums first: the body state below is not held across this loop
+  float rate = 0.f, lim = 0.f;
+  for (int a = lane; a < nu; a += 32) {
+    float da = act[a] - last[a];
+    rate += da * da;
+    float jp = qpos[7 + a];
+    lim += fmaxf(A.soft_lo[a] - jp, 0.f) + fmaxf(jp - A.soft_hi[a], 0.f);
+  }
   const bool hasb = lane < A.nb;
   const int b = hasb ? lane : 0;
   const int bid = A.body_idx[b];
@@ -222,96 +229,50 @@ __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackE
   const bool trunc = ep >= A.max_episode_length;
   const V3 g = {0.f, 0.f, -1.f};
   const float ori_err = fabsf(qapply_inv(a_quat, g).z - qapply_inv(r_quat, g).z);
-  bool term;
-  float reward;
-  if (!A.task_cfg) {
-    const bool bad_z = fabsf(a_pos.z - r_pos.z) > 0.25f;
-    const bool bad_ori = ori_err > 0.8f;
-    bool ee_bad = false;
-    for (int k = 0; k < A.nee; k++) ee_bad |= hasb && lane == A.ee_idx[k] && fabsf(rel_p.z - pos.z) > 0.25f;
-    term = bad_z || bad_ori || __any_sync(0xffffffffu, ee_bad);
-    // rewards (:200-250)
-    const float inb = 1.f / (float)A.nb;
-    float dpx = a_pos.x - r_pos.x, dpy = a_pos.y - r_pos.y, dpz = a_pos.z - r_pos.z;
-    float r = 0.5f * expf(-(dpx * dpx + dpy * dpy + dpz * dpz) / 0.09f);
-    float e = qerr(a_quat, r_quat);
-    r += 0.5f * expf(-e * e / 0.16f);
-    float ep_ = 0.f, eq_ = 0.f, el_ = 0.f, ea_ = 0.f;
-    if (hasb) {
-      float dx = rel_p.x - pos.x, dy = rel_p.y - pos.y, dz = rel_p.z - pos.z;
-      ep_ = dx * dx + dy * dy + dz * dz;
-      float qe = qerr(rel_q, quat);
-      eq_ = qe * qe;
-      const V3 cl = ldv(A.m_body_lin + 3 * (fb + b)), ca = ldv(A.m_body_ang + 3 * (fb + b));
-      el_ = (cl.x - lin.x) * (cl.x - lin.x) + (cl.y - lin.y) * (cl.y - lin.y) + (cl.z - lin.z) * (cl.z - lin.z);
-      ea_ = (ca.x - ang.x) * (ca.x - ang.x) + (ca.y - ang.y) * (ca.y - ang.y) + (ca.z - ang.z) * (ca.z - ang.z);
-    }
-    r += expf(-wsum(ep_) * inb / 0.09f);
-    r += expf(-wsum(eq_) * inb / 0.16f);
-    r += expf(-wsum(el_) * inb / 1.0f);
-    r += expf(-wsum(ea_) * inb / (3.14f * 3.14f));
-    float rate = 0.f, lim = 0.f;
-    for (int a = lane; a < nu; a += 32) {
-      float da = act[a] - last[a];
-      rate += da * da;
-      float jp = qpos[7 + a];
-      lim += fmaxf(A.soft_lo[a] - jp, 0.f) + fmaxf(jp - A.soft_hi[a], 0.f);
-    }
-    r -= 0.1f * wsum(rate);
-    r -= 10.f * wsum(lim);
-    r -= 10.f * dd.sensordata.p[(size_t)w * dd.sensordata.stride + A.self_collision_adr];
-    reward = r * A.step_dt;
-  } else {  // the configured terms (B2TrackEnvArgs.task_cfg), the episode logs and the motion errors
-    const float* W = A.weight;
-    const bool bad_z = A.term_on[0] && fabsf(a_pos.z - r_pos.z) > A.term_threshold[0];
-    const bool bad_ori = A.term_on[1] && ori_err > A.term_threshold[1];
-    bool ee_bad = false;
-    for (int k = 0; k < A.nee; k++) ee_bad |= hasb && lane == A.ee_idx[k] && fabsf(rel_p.z - pos.z) > A.term_threshold[2];
-    const bool bad_ee = A.term_on[2] && __any_sync(0xffffffffu, ee_bad);
-    term = bad_z || bad_ori || bad_ee;
-    // each term weighted, or 0 at weight 0 (not evaluated); the weights are uniform over the warp
-    const float inb = 1.f / (float)A.nb;
-    float v[B2_TRACKENV_NREW];
-    float ep_ = 0.f, eq_ = 0.f, el_ = 0.f, ea_ = 0.f;
-    if (hasb) {
-      float dx = rel_p.x - pos.x, dy = rel_p.y - pos.y, dz = rel_p.z - pos.z;
-      ep_ = dx * dx + dy * dy + dz * dz;
-      float qe = qerr(rel_q, quat);
-      eq_ = qe * qe;
-      const V3 cl = ldv(A.m_body_lin + 3 * (fb + b)), ca = ldv(A.m_body_ang + 3 * (fb + b));
-      el_ = (cl.x - lin.x) * (cl.x - lin.x) + (cl.y - lin.y) * (cl.y - lin.y) + (cl.z - lin.z) * (cl.z - lin.z);
-      ea_ = (ca.x - ang.x) * (ca.x - ang.x) + (ca.y - ang.y) * (ca.y - ang.y) + (ca.z - ang.z) * (ca.z - ang.z);
-    }
-    const float dpx = a_pos.x - r_pos.x, dpy = a_pos.y - r_pos.y, dpz = a_pos.z - r_pos.z;
-    const float e = qerr(a_quat, r_quat);
-    v[0] = W[0] != 0.f ? W[0] * expf(-div_rn(dpx * dpx + dpy * dpy + dpz * dpz, A.std2[0])) : 0.f;
-    v[1] = W[1] != 0.f ? W[1] * expf(-div_rn(e * e, A.std2[1])) : 0.f;
-    v[2] = W[2] != 0.f ? W[2] * expf(-div_rn(wsum(ep_) * inb, A.std2[2])) : 0.f;
-    v[3] = W[3] != 0.f ? W[3] * expf(-div_rn(wsum(eq_) * inb, A.std2[3])) : 0.f;
-    v[4] = W[4] != 0.f ? W[4] * expf(-div_rn(wsum(el_) * inb, A.std2[4])) : 0.f;
-    v[5] = W[5] != 0.f ? W[5] * expf(-div_rn(wsum(ea_) * inb, A.std2[5])) : 0.f;
-    float rate = 0.f, lim = 0.f;
-    for (int a = lane; a < nu; a += 32) {
-      float da = act[a] - last[a];
-      rate += da * da;
-      float jp = qpos[7 + a];
-      lim += fmaxf(A.soft_lo[a] - jp, 0.f) + fmaxf(jp - A.soft_hi[a], 0.f);
-    }
-    v[6] = W[6] != 0.f ? W[6] * wsum(rate) : 0.f;
-    v[7] = W[7] != 0.f ? W[7] * wsum(lim) : 0.f;
-    v[8] = W[8] != 0.f ? W[8] * dd.sensordata.p[(size_t)w * dd.sensordata.stride + A.self_collision_adr] : 0.f;
-    float r = 0.f;
+  const float* W = A.weight;
+  const bool bad_z = A.term_on[0] && fabsf(a_pos.z - r_pos.z) > A.term_threshold[0];
+  const bool bad_ori = A.term_on[1] && ori_err > A.term_threshold[1];
+  bool ee_bad = false;
+  for (int k = 0; k < A.nee; k++) ee_bad |= hasb && lane == A.ee_idx[k] && fabsf(rel_p.z - pos.z) > A.term_threshold[2];
+  const bool bad_ee = A.term_on[2] && __any_sync(0xffffffffu, ee_bad);
+  const bool term = bad_z || bad_ori || bad_ee;
+  // rewards (:200-250): each term weighted, or 0 at weight 0 (not evaluated); the weights are uniform over the warp
+  const float inb = 1.f / (float)A.nb;
+  float v[B2_TRACKENV_NREW];
+  float ep_ = 0.f, eq_ = 0.f, el_ = 0.f, ea_ = 0.f;
+  if (hasb) {
+    float dx = rel_p.x - pos.x, dy = rel_p.y - pos.y, dz = rel_p.z - pos.z;
+    ep_ = dx * dx + dy * dy + dz * dz;
+    float qe = qerr(rel_q, quat);
+    eq_ = qe * qe;
+    const V3 cl = ldv(A.m_body_lin + 3 * (fb + b)), ca = ldv(A.m_body_ang + 3 * (fb + b));
+    el_ = (cl.x - lin.x) * (cl.x - lin.x) + (cl.y - lin.y) * (cl.y - lin.y) + (cl.z - lin.z) * (cl.z - lin.z);
+    ea_ = (ca.x - ang.x) * (ca.x - ang.x) + (ca.y - ang.y) * (ca.y - ang.y) + (ca.z - ang.z) * (ca.z - ang.z);
+  }
+  const float dpx = a_pos.x - r_pos.x, dpy = a_pos.y - r_pos.y, dpz = a_pos.z - r_pos.z;
+  const float e = qerr(a_quat, r_quat);
+  v[0] = W[0] != 0.f ? W[0] * expf(-div_rn(dpx * dpx + dpy * dpy + dpz * dpz, A.std2[0])) : 0.f;
+  v[1] = W[1] != 0.f ? W[1] * expf(-div_rn(e * e, A.std2[1])) : 0.f;
+  v[2] = W[2] != 0.f ? W[2] * expf(-div_rn(wsum(ep_) * inb, A.std2[2])) : 0.f;
+  v[3] = W[3] != 0.f ? W[3] * expf(-div_rn(wsum(eq_) * inb, A.std2[3])) : 0.f;
+  v[4] = W[4] != 0.f ? W[4] * expf(-div_rn(wsum(el_) * inb, A.std2[4])) : 0.f;
+  v[5] = W[5] != 0.f ? W[5] * expf(-div_rn(wsum(ea_) * inb, A.std2[5])) : 0.f;
+  v[6] = W[6] != 0.f ? W[6] * wsum(rate) : 0.f;
+  v[7] = W[7] != 0.f ? W[7] * wsum(lim) : 0.f;
+  v[8] = W[8] != 0.f ? W[8] * dd.sensordata.p[(size_t)w * dd.sensordata.stride + A.self_collision_adr] : 0.f;
+  float r = 0.f;
 #pragma unroll
-    for (int k = 0; k < B2_TRACKENV_NREW; k++) r += v[k];
-    reward = r * A.step_dt;
-    const bool done_ = term || trunc;
+  for (int k = 0; k < B2_TRACKENV_NREW; k++) r += v[k];
+  const float reward = r * A.step_dt;
+  const bool done = term || trunc;
+  if (A.episode_sums) {  // the episode logs and the motion errors
     const size_t row = (size_t)w * B2_TRACKENV_NREW;
     if (lane == 0) {
 #pragma unroll
       for (int k = 0; k < B2_TRACKENV_NREW; k++) {
         const float s = A.episode_sums[row + k] + v[k] * A.step_dt;
-        if (done_) A.finished_sums[row + k] = s;
-        A.episode_sums[row + k] = done_ ? 0.f : s;
+        if (done) A.finished_sums[row + k] = s;
+        A.episode_sums[row + k] = done ? 0.f : s;
       }
       float* f = A.term_flags + (size_t)w * B2_TRACKENV_NTERM;
       f[0] = trunc ? 1.f : 0.f; f[1] = bad_z ? 1.f : 0.f; f[2] = bad_ori ? 1.f : 0.f; f[3] = bad_ee ? 1.f : 0.f;
@@ -319,14 +280,13 @@ __global__ void b2_trackenv_post1_kernel(DevData dd, int nu, int nbody, B2TrackE
     // motion errors: a done env hands over those of the last step's compute and takes new ones in post2, after the
     // forward; every other env takes them here, at its frame before the clip steps
     float* mm = A.motion_metrics + (size_t)w * B2_TRACKENV_NMETRIC;
-    if (done_) {
+    if (done) {
       if (lane < B2_TRACKENV_NMETRIC) A.finished_metrics[(size_t)w * B2_TRACKENV_NMETRIC + lane] = mm[lane];
     } else {
       const float* qvel = dd.qvel.p + (size_t)w * dd.qvel.stride;
       motion_errors(A, lane, hasb, b, ts, org, pos, quat, lin, ang, rel_p, rel_q, qpos, qvel, nu, mm);
     }
   }
-  const bool done = term || trunc;
   __syncwarp();  // every lane has read the pre-reset state
   if (lane == 0) {
     A.reward[w] = reward; A.terminated[w] = term; A.truncated[w] = trunc;
@@ -386,7 +346,7 @@ __global__ void b2_trackenv_post2_kernel(DevData dd, int nu, int nbody, B2TrackE
   const Q r_quat = bcastq(quat, A.anchor);
   // motion errors of a done env against its reset state, at the frame before the clip stepped and the targets of the
   // last command update (the reference's compute runs _update_metrics before _update_command)
-  if (A.task_cfg && (A.terminated[w] || A.truncated[w])) {
+  if (A.episode_sums && (A.terminated[w] || A.truncated[w])) {
     const float* lv = dd.link_vel_w.p + (size_t)w * dd.link_vel_w.stride + 6 * bid;
     const V3 rel_p = ldv(A.body_pos_rel + 3 * ((size_t)w * A.nb + b));
     const Q rel_q = ldq(A.body_quat_rel + 4 * ((size_t)w * A.nb + b));
@@ -406,12 +366,11 @@ __global__ void b2_trackenv_post2_kernel(DevData dd, int nu, int nbody, B2TrackE
     bq[0] = rq.w; bq[1] = rq.x; bq[2] = rq.y; bq[3] = rq.z;
   }
   // interval push (push_by_setting_velocity, events.py:127-143) from the root's link velocity and orientation
-  const bool push_on = !A.task_cfg || A.push_on;
-  const float* pr = A.task_cfg ? A.push_range : A.vel_range;
+  const float* pr = A.push_range;
   float tl = A.push_time_left[w] - A.step_dt;
-  const bool push = push_on && tl <= 0.f;
+  const bool push = A.push_on && tl <= 0.f;
   if (push) tl = P[6] * (A.push_hi - A.push_lo) + A.push_lo;
-  if (lane == 0 && push_on) {
+  if (lane == 0 && A.push_on) {
     if (push) {
       const float* rv = dd.link_vel_w.p + (size_t)w * dd.link_vel_w.stride + 6 * A.root_body;
       float v[6];
@@ -425,7 +384,7 @@ __global__ void b2_trackenv_post2_kernel(DevData dd, int nu, int nbody, B2TrackE
   }
   // observations (tracking_env_cfg.py:88-150): policy group with uniform noise, critic group privileged; without
   // state estimation the policy group has no anchor position and no base linear velocity
-  const bool se = !A.task_cfg || A.policy_state_estimation, noisy = !A.task_cfg || A.policy_corruption;
+  const bool se = A.policy_state_estimation, noisy = A.policy_corruption;
   const int NP = se ? 5 * nu + 15 : 5 * nu + 9, NC = 5 * nu + 15 + 9 * A.nb;
   const int pj = NP - 3 * nu;            // policy: joint pos, joint vel, last action
   float* o = A.obs + (size_t)w * NP;

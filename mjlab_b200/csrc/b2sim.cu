@@ -1096,30 +1096,23 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
        !args->terrain_level_mean || args->rows < 1 || args->cols < 1))
     return fail("b2_velenv_post: the terrain curriculum needs env_origins, terrain_origins, terrain_levels, "
                 "terrain_types, terrain_level_mean and rows, cols >= 1");
-  if (args->rewards) {
-    const B2VelEnvArgs& a = *args;
-    const float* W = a.weight;
-    const bool feet_ok = a.n_air >= 0 && a.n_air <= 32 && a.n_slide >= 0 && a.n_slide <= 32 && a.n_clear >= 0 &&
-                         a.n_clear <= 32 && a.root_body >= 0 && a.root_body < s->hm.nbody;
-    if (!feet_ok || (W[0] != 0.f && (!a.air_sensor_adr || !a.air_time || !a.contact_time || !a.last_air_time)) ||
-        (W[1] != 0.f && (!a.slide_sensor_adr || !a.slide_geom || !a.slide_body)) ||
-        (W[2] != 0.f && (!a.clear_geom || !a.clear_body)) || (a.episode_sums && !a.finished_sums))
-      return fail("b2_velenv_post: the reward terms need at most 32 feet each, a valid root_body, the arrays of "
-                  "every term with a non-zero weight, and finished_sums beside episode_sums");
-  }
-  if (args->command_cfg && !(args->resample_lo > 0.f && args->resample_span >= 0.f && args->ang_lo <= args->ang_hi))
+  const B2VelEnvArgs& a = *args;
+  const float* W = a.weight;
+  const bool feet_ok = a.n_air >= 0 && a.n_air <= 32 && a.n_slide >= 0 && a.n_slide <= 32 && a.n_clear >= 0 &&
+                       a.n_clear <= 32 && a.root_body >= 0 && a.root_body < s->hm.nbody;
+  if (!feet_ok || (W[0] != 0.f && (!a.air_sensor_adr || !a.air_time || !a.contact_time || !a.last_air_time)) ||
+      (W[1] != 0.f && (!a.slide_sensor_adr || !a.slide_geom || !a.slide_body)) ||
+      (W[2] != 0.f && (!a.clear_geom || !a.clear_body)))
+    return fail("b2_velenv_post: the reward terms need at most 32 feet each, a valid root_body and the arrays of "
+                "every term with a non-zero weight");
+  if (!(a.resample_lo > 0.f && a.resample_span >= 0.f && a.ang_lo <= a.ang_hi))
     return fail("b2_velenv_post: the command needs resample_lo > 0, resample_span >= 0 and ang_lo <= ang_hi");
-  if (args->n_stage < 0 || args->n_stage > B2_VELENV_NSTAGE || (args->n_stage > 0 && !args->step_counter))
+  if (a.n_stage < 0 || a.n_stage > B2_VELENV_NSTAGE || (a.n_stage > 0 && !a.step_counter))
     return fail("b2_velenv_post: the command curriculum needs 0 <= n_stage <= B2_VELENV_NSTAGE and a step_counter");
-  if (args->metric_xy && (!args->metric_yaw || !args->finished_metrics || !(args->metric_steps > 0.f)))
-    return fail("b2_velenv_post: the command metrics need metric_yaw, finished_metrics and metric_steps > 0");
-  B2VelEnvArgs a = *args;
-  if (!a.command_cfg) {  // the ranges, widths and timer of velocity_env_cfg.py:66-83
-    const float mid[4] = {0.f, 0.f, 0.f, 0.f}, half[4] = {1.f, 0.5f, 1.f, 3.14159265358979f};
-    for (int k = 0; k < 4; k++) { a.cmd_mid[k] = mid[k]; a.cmd_half[k] = half[k]; }
-    a.ang_lo = -1.f; a.ang_hi = 1.f;
-    a.heading_stiffness = 0.5f; a.rel_standing = 0.1f; a.resample_lo = 3.f; a.resample_span = 5.f;
-  }
+  if (!a.episode_sums || !a.finished_sums || !a.posture_inv_std2 || !a.metric_xy || !a.metric_yaw ||
+      !a.finished_metrics || !(a.metric_steps > 0.f))
+    return fail("b2_velenv_post: needs episode_sums, finished_sums, posture_inv_std2, metric_xy, metric_yaw, "
+                "finished_metrics and metric_steps > 0");
   DeviceGuard guard(s->device);
   b2_velenv_post_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(  // one warp per environment
       s->hd, s->hm.nq, s->hm.nv, s->hm.nu, a);
@@ -1139,7 +1132,8 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
   return 0;
 }
 
-static int trackenv_check(b2_sim* s, const B2TrackEnvArgs* a) {
+// `settings`: also the task settings and the episode logs, which post1 and post2 read and bins does not
+static int trackenv_check(b2_sim* s, const B2TrackEnvArgs* a, bool settings) {
   if (!s || !a) return fail("b2_trackenv: bad arguments");
   if (s->hm.nq != s->hm.nu + 7 || s->hm.nv != s->hm.nu + 6)
     return fail("b2_trackenv: expects one floating base plus nu actuated hinge joints");
@@ -1153,22 +1147,22 @@ static int trackenv_check(b2_sim* s, const B2TrackEnvArgs* a) {
       (a->nbins < 1 || a->adaptive_kernel_size < 1 || !a->adaptive_kernel || !a->cdf || !a->bin_fail_ema ||
        !a->bin_fail_cur || !a->metrics))
     return fail("b2_trackenv: the adaptive sampler needs nbins >= 1, a kernel of size >= 1 and its five arrays");
-  if (a->task_cfg) {
-    bool ok = a->episode_sums && a->finished_sums && a->term_flags && a->motion_metrics && a->finished_metrics;
-    for (int k = 0; k < 6; k++) ok = ok && a->std2[k] > 0.f && a->std2[k] < INFINITY;
-    for (int k = 0; k < 3; k++)
-      ok = ok && (a->term_on[k] == 0 || (a->term_on[k] == 1 && a->term_threshold[k] > 0.f && a->term_threshold[k] < INFINITY));
-    for (int k = 0; k < 6; k++)
-      ok = ok && a->pose_range[2 * k] <= a->pose_range[2 * k + 1] && a->vel_range[2 * k] <= a->vel_range[2 * k + 1] &&
-           (!a->push_on || a->push_range[2 * k] <= a->push_range[2 * k + 1]);
-    if (!ok)
-      return fail("b2_trackenv: task_cfg needs the five log arrays, finite stds^2 > 0, finite thresholds > 0 on the "
-                  "terms that are on, and lo <= hi in every range");
-  }
+  if (!settings) return 0;
+  const int logs = !!a->episode_sums + !!a->finished_sums + !!a->term_flags + !!a->motion_metrics + !!a->finished_metrics;
+  bool ok = logs == 0 || logs == 5;
+  for (int k = 0; k < 6; k++) ok = ok && a->std2[k] > 0.f && a->std2[k] < INFINITY;
+  for (int k = 0; k < 3; k++)
+    ok = ok && (a->term_on[k] == 0 || (a->term_on[k] == 1 && a->term_threshold[k] > 0.f && a->term_threshold[k] < INFINITY));
+  for (int k = 0; k < 6; k++)
+    ok = ok && a->pose_range[2 * k] <= a->pose_range[2 * k + 1] && a->vel_range[2 * k] <= a->vel_range[2 * k + 1] &&
+         (!a->push_on || a->push_range[2 * k] <= a->push_range[2 * k + 1]);
+  if (!ok)
+    return fail("b2_trackenv: needs the five log arrays all set or all null, finite stds^2 > 0, finite thresholds > 0 "
+                "on the terms that are on, and lo <= hi in every range");
   return 0;
 }
 int b2_trackenv_post1(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
-  if (trackenv_check(s, args)) return 1;
+  if (trackenv_check(s, args, true)) return 1;
   DeviceGuard guard(s->device);
   b2_trackenv_post1_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(s->hd, s->hm.nu, s->hm.nbody, *args);
   s->launches++;
@@ -1176,7 +1170,7 @@ int b2_trackenv_post1(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   return 0;
 }
 int b2_trackenv_post2(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
-  if (trackenv_check(s, args)) return 1;
+  if (trackenv_check(s, args, true)) return 1;
   DeviceGuard guard(s->device);
   b2_trackenv_post2_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(s->hd, s->hm.nu, s->hm.nbody, *args);
   s->launches++;
@@ -1184,7 +1178,7 @@ int b2_trackenv_post2(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   return 0;
 }
 int b2_trackenv_bins(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
-  if (trackenv_check(s, args)) return 1;
+  if (trackenv_check(s, args, false)) return 1;
   if (args->adaptive != B2_START_ADAPTIVE) return fail("b2_trackenv_bins: the args do not select the adaptive sampler");
   DeviceGuard guard(s->device);
   b2_trackenv_bins_kernel<<<1, b2t::kBinThreads, 0, (cudaStream_t)stream>>>(*args);

@@ -157,14 +157,6 @@ class TrackingEnvCfg:
     if not self.episode_length_s > 0:
       raise ValueError(f"episode_length_s must be positive, not {self.episode_length_s}")
 
-  def is_base_task(self) -> bool:
-    """True when every task setting is the base task's (the fused kernels' literal terms) and no log is asked for."""
-    f = lambda r: None if r is None else tuple(tuple(float(x) for x in p) for p in r)
-    return (self.rewards == TrackingRewardsCfg() and self.terminations == TrackingTerminationsCfg()
-            and f(self.pose_range) == POSE_RANGE and f(self.velocity_range) == VELOCITY_RANGE
-            and f(self.push_velocity_range) == VELOCITY_RANGE and self.policy_state_estimation
-            and self.policy_corruption and not self.episode_logs)
-
 
 _NO_RSI = ((0.0, 0.0),) * 6  # an empty pose_range / velocity_range dict of MotionCommandCfg: every offset 0
 _PLAY = dict(policy_corruption=False, push_velocity_range=None, pose_range=_NO_RSI, velocity_range=_NO_RSI,
@@ -310,7 +302,6 @@ class TrackingFlatEnv:
     cfg, n = self.cfg, self.num_envs
     f32 = dict(dtype=torch.float32, device=self.device)
     rc, tc = cfg.rewards, cfg.terminations
-    self.task_cfg = not cfg.is_base_task()  # the fused kernels' configured path (B2TrackEnvArgs.task_cfg)
     self.reward_weights = [float(getattr(rc, t)) for t in REWARD_TERMS]
     self.reward_stds = [float(getattr(rc, t + "_std")) for t in TRACKING_TERMS]
     self.term_thresholds = [getattr(tc, t) for t in TERMINATION_TERMS[1:]]
@@ -601,23 +592,22 @@ class TrackingFlatEnv:
       ptr.update(sampler)
       A.adaptive_alpha, A.adaptive_uniform_ratio = self.cfg.adaptive_alpha, self.cfg.adaptive_uniform_ratio
       A.nbins, A.adaptive_kernel_size = self.bin_count, self.cfg.adaptive_kernel_size
-    if self.task_cfg:
+    A.weight[:] = self.reward_weights
+    A.std2[:] = [s**2 for s in self.reward_stds]  # (the fp32 value of the double the torch path divides by)
+    for k, v in enumerate(self.term_thresholds):
+      A.term_on[k], A.term_threshold[k] = v is not None, 0.0 if v is None else v
+    if self.cfg.push_velocity_range is not None:
+      A.push_on = 1
+      for k in range(6):
+        A.push_range[2 * k], A.push_range[2 * k + 1] = self.cfg.push_velocity_range[k]
+    A.policy_state_estimation, A.policy_corruption = self.cfg.policy_state_estimation, self.cfg.policy_corruption
+    if self.cfg.episode_logs:
       logs = dict(episode_sums=self.episode_sums, finished_sums=self.finished_sums, term_flags=self.term_flags,
                   motion_metrics=self.motion_metrics, finished_metrics=self.finished_metrics)
       for k, t in logs.items():
         assert t.is_contiguous() and t.dtype == torch.float32, k
         setattr(A, k, t.data_ptr())
       ptr.update(logs)
-      A.task_cfg = 1
-      A.weight[:] = self.reward_weights
-      A.std2[:] = [s**2 for s in self.reward_stds]  # (the fp32 value of the double the torch path divides by)
-      for k, v in enumerate(self.term_thresholds):
-        A.term_on[k], A.term_threshold[k] = v is not None, 0.0 if v is None else v
-      if self.cfg.push_velocity_range is not None:
-        A.push_on = 1
-        for k in range(6):
-          A.push_range[2 * k], A.push_range[2 * k + 1] = self.cfg.push_velocity_range[k]
-      A.policy_state_estimation, A.policy_corruption = self.cfg.policy_state_estimation, self.cfg.policy_corruption
     self._native_args = A
     self._keep = ptr
 
@@ -708,10 +698,10 @@ class TrackingFlatEnv:
     self.last_action.copy_(action)
     done = terminated | truncated
     self.log_row.copy_(torch.stack([reward, terminated.float(), truncated.float()], dim=1))
-    # episode logs (RewardManager / TerminationManager), kept where the fused kernels keep them (task_cfg): a done
+    # episode logs (RewardManager / TerminationManager), kept only with episode_logs, as on the fused kernels: a done
     # env's sums end their episode
     dk = done.unsqueeze(1)
-    if self.task_cfg:
+    if cfg.episode_logs:
       sums = self.episode_sums + torch.stack(vals, dim=1) * self.step_dt
       self.finished_sums.copy_(torch.where(dk, sums, self.finished_sums))
       self.episode_sums.copy_(torch.where(dk, 0.0, sums))
@@ -736,7 +726,7 @@ class TrackingFlatEnv:
     self._done_buf.copy_(done | ended)
     self.sim.forward(env_mask=self._done_buf)
     # a done env's motion errors: its reset state against the frame before the clip stepped and the stale targets
-    if self.task_cfg:
+    if cfg.episode_logs:
       e = self._motion_errors((self.time_steps - 1).clamp(min=0), *self._robot_bodies())
       self.motion_metrics.copy_(torch.where(dk, e, self.motion_metrics))
     self._update_command()

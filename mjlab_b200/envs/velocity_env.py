@@ -364,10 +364,8 @@ class VelocityFlatEnv:
     # common_step_counter (manager_based_rl_env.py:117); it only advances with the command curriculum on, the one
     # thing that reads it
     self.common_step_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-    self.posture_inv_std2 = None
-    if cfg.posture_std is not None:
-      std = np.asarray(resolve_posture_std(cfg.posture_std, joint_names), dtype=np.float64)
-      self.posture_inv_std2 = torch.tensor(1.0 / std ** 2, **f32)
+    std = [0.3] * len(joint_names) if cfg.posture_std is None else resolve_posture_std(cfg.posture_std, joint_names)
+    self.posture_inv_std2 = torch.tensor(1.0 / np.asarray(std, dtype=np.float64) ** 2, **f32)
     self.metric_steps = _float32(cc.resampling_time_range[1] / self.step_dt)
     self.metric_xy = torch.zeros(n, **f32)
     self.metric_yaw = torch.zeros(n, **f32)
@@ -465,7 +463,7 @@ class VelocityFlatEnv:
       0.0 if v is None else v for v in (rc.target_height, rc.std, rc.tanh_mult))
     a.air_continuous, a.air_hard_scale = rc.reward_mode == "continuous", rc.command_scale_type == "hard"
     a.n_air, a.n_slide, a.n_clear = len(self._air_adr), len(self._slide_adr), len(self._clear_geom)
-    a.root_body, a.rewards = self._root_body, 1
+    a.root_body = self._root_body
     cc = self.cfg.command
     for k, (mid, half) in enumerate(self._cmd_mid_half):
       a.cmd_mid[k], a.cmd_half[k] = mid, half
@@ -473,16 +471,14 @@ class VelocityFlatEnv:
     a.heading_stiffness, a.rel_standing = cc.heading_control_stiffness, cc.rel_standing_envs
     lo_t, hi_t = cc.resampling_time_range
     a.resample_lo, a.resample_span = lo_t, _float32(np.float32(hi_t) - np.float32(lo_t))
-    a.command_cfg = 1
     a.n_stage = len(self._stages)
     for s, (step, mid, half, lo, hi) in enumerate(self._stages):
       a.stage_step[s], a.stage_mid[s], a.stage_half[s], a.stage_lo[s], a.stage_hi[s] = step, mid, half, lo, hi
     for name, t in (("step_counter", self.common_step_counter), ("posture_inv_std2", self.posture_inv_std2),
                     ("metric_xy", self.metric_xy), ("metric_yaw", self.metric_yaw),
                     ("finished_metrics", self.finished_metrics)):
-      if t is not None:
-        assert t.is_contiguous()
-        setattr(a, name, t.data_ptr())
+      assert t.is_contiguous()
+      setattr(a, name, t.data_ptr())
     a.metric_steps = self.metric_steps
     self._native_args = a
 
@@ -576,10 +572,8 @@ class VelocityFlatEnv:
 
   def _posture(self, jp: torch.Tensor) -> torch.Tensor:
     """The pose reward (posture, envs/mdp/rewards.py:73-104): exp(-mean(d^2 / std^2)) with the per-joint widths of
-    posture_std, else exp(-mean(d^2) / 0.3^2)."""
+    posture_std (0.3 for every joint without one)."""
     d2 = (jp - self.default_joint_pos) ** 2
-    if self.posture_inv_std2 is None:
-      return torch.exp(-d2.mean(1) / 0.09)
     return torch.exp(-(d2 * self.posture_inv_std2).mean(1))
 
   def _update_command(self, done: torch.Tensor, U: torch.Tensor, metrics: bool = True) -> None:

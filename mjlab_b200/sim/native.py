@@ -67,11 +67,10 @@ class B2VelEnvArgs(ctypes.Structure):
     + [(n, ctypes.c_void_p) for n in (
       "air_sensor_adr", "slide_sensor_adr", "slide_geom", "slide_body", "clear_geom", "clear_body", "air_time",
       "contact_time", "last_air_time", "episode_sums", "finished_sums")]
-    + [("rewards", ctypes.c_int32)]
     + [(n, ctypes.c_float * 4) for n in ("cmd_mid", "cmd_half")]
     + [(n, ctypes.c_float) for n in ("ang_lo", "ang_hi", "heading_stiffness", "rel_standing", "resample_lo",
                                      "resample_span")]
-    + [(n, ctypes.c_int32) for n in ("command_cfg", "n_stage")]
+    + [("n_stage", ctypes.c_int32)]
     + [("stage_step", ctypes.c_int32 * VELENV_NSTAGE)]
     + [(n, ctypes.c_float * VELENV_NSTAGE) for n in ("stage_mid", "stage_half", "stage_lo", "stage_hi")]
     + [(n, ctypes.c_void_p) for n in ("step_counter", "posture_inv_std2", "metric_xy", "metric_yaw",
@@ -93,7 +92,7 @@ class B2TrackEnvArgs(ctypes.Structure):
     + [(n, ctypes.c_void_p) for n in ("adaptive_kernel", "cdf", "bin_fail_ema", "bin_fail_cur", "metrics")]
     + [(n, ctypes.c_float) for n in ("adaptive_alpha", "adaptive_uniform_ratio")]
     + [(n, ctypes.c_int32) for n in ("nbins", "adaptive", "adaptive_kernel_size")]
-    + [("task_cfg", ctypes.c_int32), ("weight", ctypes.c_float * 9), ("std2", ctypes.c_float * 6),
+    + [("weight", ctypes.c_float * 9), ("std2", ctypes.c_float * 6),
        ("term_threshold", ctypes.c_float * 3), ("term_on", ctypes.c_int32 * 3), ("push_range", ctypes.c_float * 12)]
     + [(n, ctypes.c_int32) for n in ("push_on", "policy_state_estimation", "policy_corruption")]
     + [(n, ctypes.c_void_p) for n in ("episode_sums", "finished_sums", "term_flags", "motion_metrics",

@@ -324,8 +324,8 @@ def test_disabled_adaptive_sampling_starts_every_episode_at_frame_zero(clip, mon
     e.close()
 
 
-def test_without_a_motion_file_the_sampler_fields_stay_zero(monkeypatch):
-  """motion_file=None: the argument block's sampler tail is all zero, and a run with that tail zeroed explicitly
+def test_without_a_motion_file_the_sampler_fields_are_zero(monkeypatch):
+  """motion_file=None: the argument block's sampler fields are all zero, and a run with those fields zeroed explicitly
   gives bit-identical outputs."""
   cfg = dict(num_envs=3, decimation=1, episode_length_s=0.015, clip_frames=4, native_mdp=True)
   a = _emul_env(monkeypatch, **dict(cfg))
@@ -333,8 +333,8 @@ def test_without_a_motion_file_the_sampler_fields_stay_zero(monkeypatch):
   a._native_setup()
   b._native_setup()
   A = b._native_args
-  tail = native.B2TrackEnvArgs.adaptive_kernel.offset
-  ctypes.memset(ctypes.addressof(A) + tail, 0, ctypes.sizeof(A) - tail)
+  first, last = native.B2TrackEnvArgs.adaptive_kernel, native.B2TrackEnvArgs.adaptive_kernel_size
+  ctypes.memset(ctypes.addressof(A) + first.offset, 0, last.offset + last.size - first.offset)
   for f in ("adaptive_kernel", "cdf", "bin_fail_ema", "bin_fail_cur", "metrics", "adaptive_alpha",
             "adaptive_uniform_ratio", "nbins", "adaptive", "adaptive_kernel_size"):
     assert not getattr(a._native_args, f), f

@@ -142,6 +142,8 @@ def test_curriculum_needs_a_terrain_grid():
 
 
 def test_post_kernel_refuses_curriculum_without_tables():
+  """The curriculum without its tables is refused, and so are a zeroed command block and a block without the arrays
+  every step writes."""
   sys.path.insert(0, str(refload.ROOT / "tests" / "emul"))
   from engine import load_emul_library
 
@@ -149,10 +151,13 @@ def test_post_kernel_refuses_curriculum_without_tables():
 
   lib = load_emul_library(())
   e = native.Engine(lib, load_compiled("go1_flat"), 1)
-  a = native.B2VelEnvArgs()
-  a.curriculum, a.rows, a.cols = 1, 10, 20
-  assert lib.b2_velenv_post(e.h, ctypes.byref(a), None) != 0
-  assert b"terrain curriculum" in lib.b2_last_error()
+  curriculum, zeroed, no_arrays = native.B2VelEnvArgs(), native.B2VelEnvArgs(), native.B2VelEnvArgs()
+  curriculum.curriculum, curriculum.rows, curriculum.cols = 1, 10, 20
+  no_arrays.resample_lo = 3.0
+  for a, match in ((curriculum, b"terrain curriculum"), (zeroed, b"the command needs"),
+                   (no_arrays, b"needs episode_sums")):
+    assert lib.b2_velenv_post(e.h, ctypes.byref(a), None) != 0
+    assert match in lib.b2_last_error()
   e.close()
 
 

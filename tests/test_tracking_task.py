@@ -3,7 +3,7 @@ the RSI / push ranges, the two policy-group switches, tracking_task_cfg and the 
 termination_log, command_log).
 
 * The presets against the reference's cfg classes (read through tests/ref_tracking_cfgs.py under tests/ref_runner.py).
-* The fused kernels' configured path (B2TrackEnvArgs.task_cfg) against the torch path on one saved state per step
+* The fused kernels' configured terms and logs against the torch path on one saved state per step
   (test_mdp_kernels.Harness): emulated backend in the CPU suite, the H100 under -m gpu.
 * The play tasks: never truncated, frame-0 starts without RSI offsets, no push, policy = critic on the shared terms.
 * Refused configurations, the C ABI of the appended block.
@@ -105,13 +105,13 @@ CASES.update({f"weight0_{t}": dict(rewards=R(**{t: 0.0})) for t in te.REWARD_TER
 
 @pytest.mark.parametrize("case", list(CASES))
 @pytest.mark.parametrize("backend", BACKENDS)
-def test_configured_path_matches_torch(backend, case, monkeypatch):
+def test_configured_terms_match_torch(backend, case, monkeypatch):
   big = backend == "cuda"
   cfg = dict(num_envs=1024 if big else 8, episode_length_s=0.3 if big else 0.06, clip_frames=30 if big else 6,
              push_interval_s=(0.05, 0.15) if big else (0.02, 0.06))
   cfg.update({"episode_logs": True, **CASES[case]})
   H = _harness(backend, monkeypatch, **cfg)
-  assert H.env.task_cfg and H.env._native_args.task_cfg == 1
+  assert all(getattr(H.env._native_args, f) for f in LOGS)
   _rollout(H, 30 if big else 5, seed=11)
   H.report(f"configured {case}")
   c = H.counts
@@ -396,12 +396,14 @@ def test_inconsistent_block_is_refused(monkeypatch):
   H = _harness("emul", monkeypatch, num_envs=2, clip_frames=4, episode_length_s=1.0, episode_logs=True)
   env = H.env
   A = env._native_args
-  for field, bad in (("term_flags", None), ("finished_metrics", None)):
-    keep = getattr(A, field)
-    setattr(A, field, bad)
+  logs = {f: getattr(A, f) for f in LOGS}
+  for nulls in (["term_flags"], ["finished_metrics"], LOGS[1:]):  # some log arrays set, some null
+    for f in nulls:
+      setattr(A, f, None)
     with pytest.raises(RuntimeError):
       env._mdp_native(torch.zeros(2, env.nu), torch.rand(2, 48 + 4 * env.nu))
-    setattr(A, field, keep)
+    for f, p in logs.items():
+      setattr(A, f, p)
   for arr, k, bad in (("std2", 3, 0.0), ("term_threshold", 1, -1.0), ("push_range", 0, 5.0)):
     keep = getattr(A, arr)[k]
     getattr(A, arr)[k] = bad
@@ -412,9 +414,9 @@ def test_inconsistent_block_is_refused(monkeypatch):
   env.close()
 
 
-def test_logs_need_episode_logs(monkeypatch):
+def test_log_methods_need_episode_logs(monkeypatch):
   H = _harness("emul", monkeypatch, num_envs=2, clip_frames=4)
-  assert not H.env.task_cfg and H.env._native_args.task_cfg == 0
+  assert not any(getattr(H.env._native_args, f) for f in LOGS)
   for f in (H.env.reward_log, H.env.termination_log, H.env.command_log):
     with pytest.raises(RuntimeError):
       f()
