@@ -311,6 +311,44 @@ int b2_trackenv_post2(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream
  * order (run-to-run deterministic). */
 int b2_trackenv_bins(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream);
 
+/* ---- clip, scale and history of the observation groups (the reference's ObservationManager,
+ * managers/observation_manager.py:153-188, with its CircularBuffer, utils/buffers/circular_buffer.py) ---------------
+ * Runs after the env's post kernel (b2_velenv_post, b2_trackenv_post2) on the group rows it wrote, one launch for every
+ * group.  For element j of term t of group g in env w:
+ *   v = frame[w][src + j], clamped to [lo, hi] when clip = 1, then times scale[t.scale + j] when t.scale >= 0 (one
+ *   IEEE fp32 product, subnormals kept);
+ *   the term's frames sit in out[w] at columns dst + k stride + j, k = 0 (oldest) .. max(frames, 1) - 1 (newest):
+ *   every frame moves one slot older and v is written into the newest; an env whose terminated or truncated byte is
+ *   set (the reference's reset_buf) gets v in every slot.
+ * The terms tile the frame row in order (src of term 0 is 0, each next src is the previous src + dim, the last ends at
+ * frame_width), and their frames tile the out row: every column of out is written by exactly one element. */
+#define B2_OBSHIST_NTERM 16  /* terms per group */
+#define B2_OBSHIST_NGROUP 2  /* groups per launch (policy, critic) */
+typedef struct B2ObsHistTerm {
+  int32_t src;                    /* first column of the term in the frame row */
+  int32_t dim;                    /* elements of one frame of the term, >= 1 */
+  int32_t frames;                 /* history length, >= 0; 0: no history (one frame, as 1) */
+  int32_t dst;                    /* column of the term's oldest frame in the out row */
+  int32_t stride;                 /* columns from one frame of the term to the next */
+  int32_t scale;                  /* offset of the term's dim factors in B2ObsHistArgs.scale; -1: not scaled */
+  int32_t clip;                   /* 1: clamp to [lo, hi] (finite, lo <= hi); 0: no clip */
+  float lo, hi;
+} B2ObsHistTerm;
+typedef struct B2ObsHistGroup {
+  const float* frame;             /* [n][frame_width] the group's row as the post kernel wrote it (noise applied) */
+  float* out;                     /* [n][out_width] in/out: the group's output, which is its history */
+  int32_t frame_width, out_width, nterm;
+  B2ObsHistTerm term[B2_OBSHIST_NTERM];
+} B2ObsHistGroup;
+typedef struct B2ObsHistArgs {
+  const unsigned char* terminated; /* [n] this env step's terminations */
+  const unsigned char* truncated;  /* [n] this env step's time-outs */
+  const float* scale;             /* [nscale] per-element factors of the scaled terms; may be null when nscale = 0 */
+  int32_t nscale, ngroup;         /* 1 <= ngroup <= B2_OBSHIST_NGROUP */
+  B2ObsHistGroup group[B2_OBSHIST_NGROUP];
+} B2ObsHistArgs;
+int b2_obs_history(b2_sim* sim, const B2ObsHistArgs* args, void* cuda_stream);
+
 /* Diagnostics (synchronises `cuda_stream`). */
 int b2_stats(b2_sim* sim, void* cuda_stream, B2Stats* out);
 /* Number of kernels this library has launched for `sim` since creation. */

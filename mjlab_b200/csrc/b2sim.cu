@@ -15,6 +15,7 @@
 #include "b2_tables.h"
 #include "b2_env.cuh"
 #include "b2_trackenv.cuh"
+#include "b2_obshist.cuh"
 
 static thread_local std::string g_err;
 static int fail(const std::string& msg) {
@@ -1182,6 +1183,51 @@ int b2_trackenv_bins(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   if (args->adaptive != B2_START_ADAPTIVE) return fail("b2_trackenv_bins: the args do not select the adaptive sampler");
   DeviceGuard guard(s->device);
   b2_trackenv_bins_kernel<<<1, b2t::kBinThreads, 0, (cudaStream_t)stream>>>(*args);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+static int obshist_check(b2_sim* s, const B2ObsHistArgs* a) {
+  if (!s || !a) return fail("b2_obs_history: bad arguments");
+  if (!a->terminated || !a->truncated || a->ngroup < 1 || a->ngroup > B2_OBSHIST_NGROUP || a->nscale < 0 ||
+      (a->nscale > 0 && !a->scale))
+    return fail("b2_obs_history: needs terminated, truncated, 1 <= ngroup <= B2_OBSHIST_NGROUP and the scale row");
+  for (int g = 0; g < a->ngroup; g++) {
+    const B2ObsHistGroup& G = a->group[g];
+    if (!G.frame || !G.out || G.frame_width < 1 || G.out_width < 1 || G.nterm < 1 || G.nterm > B2_OBSHIST_NTERM)
+      return fail("b2_obs_history: a group needs its frame and out rows, widths >= 1 and 1 <= nterm <= B2_OBSHIST_NTERM");
+    std::vector<char> seen(G.out_width, 0);
+    long long next = 0, covered = 0;
+    for (int t = 0; t < G.nterm; t++) {
+      const B2ObsHistTerm& T = G.term[t];
+      if (T.src != next || T.dim < 1 || T.frames < 0 || T.stride < 0 || T.scale < -1 ||
+          (T.scale >= 0 && (long long)T.scale + T.dim > a->nscale) || (T.clip != 0 && T.clip != 1) ||
+          (T.clip && !(T.lo <= T.hi && T.lo > -INFINITY && T.hi < INFINITY)))
+        return fail("b2_obs_history: a term needs dim >= 1, frames >= 0, its scale factors inside the scale row and a "
+                    "finite clip with lo <= hi, and the terms must follow each other through the frame row");
+      next += T.dim;
+      const int H = T.frames > 1 ? T.frames : 1;
+      for (int k = 0; k < H; k++)
+        for (int j = 0; j < T.dim; j++) {
+          const long long c = (long long)T.dst + (long long)k * T.stride + j;
+          if (c < 0 || c >= G.out_width || seen[c])
+            return fail("b2_obs_history: the terms' frames must tile the out row (a column outside it or written twice)");
+          seen[c] = 1;
+          covered++;
+        }
+    }
+    if (next != G.frame_width || covered != G.out_width)
+      return fail("b2_obs_history: the terms' sizes do not add up to frame_width and out_width");
+  }
+  return 0;
+}
+int b2_obs_history(b2_sim* s, const B2ObsHistArgs* args, void* stream) {
+  if (obshist_check(s, args)) return 1;
+  long long total = 0;
+  for (int g = 0; g < args->ngroup; g++) total += (long long)s->nworld * args->group[g].frame_width;
+  DeviceGuard guard(s->device);
+  b2_obs_history_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(s->nworld, *args);
   s->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

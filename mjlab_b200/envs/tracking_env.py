@@ -35,6 +35,7 @@ import torch.nn.functional as F
 from mjlab_b200.asset_zoo import g1, load_compiled
 from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply, quat_apply_inverse, quat_mul
 from mjlab_b200.envs.motion import MotionClip
+from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.envs.velocity_env import _resolve
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg, native
 
@@ -52,6 +53,17 @@ TERMINATION_TERMS = ("time_out", "anchor_pos", "anchor_ori", "ee_body_pos")
 METRICS = ("error_anchor_pos", "error_anchor_rot", "error_anchor_lin_vel", "error_anchor_ang_vel", "error_body_pos",
            "error_body_rot", "error_body_lin_vel", "error_body_ang_vel", "error_joint_pos", "error_joint_vel")
 INT32_MAX = 2**31 - 1
+
+
+def obs_terms(nu: int, nb: int, state_estimation: bool = True) -> dict:
+  """{group: [(term, elements), ...]} in frame order (tracking_env_cfg.py:88-150); without state estimation the policy
+  group has no motion_anchor_pos_b and no base_lin_vel."""
+  policy = [("command", 2 * nu), ("motion_anchor_pos_b", 3), ("motion_anchor_ori_b", 6), ("base_lin_vel", 3),
+            ("base_ang_vel", 3), ("joint_pos", nu), ("joint_vel", nu), ("actions", nu)]
+  critic = policy[:3] + [("body_pos", 3 * nb), ("body_ori", 6 * nb)] + policy[3:]
+  if not state_estimation:
+    policy = [t for t in policy if t[0] not in ("motion_anchor_pos_b", "base_lin_vel")]
+  return {"policy": policy, "critic": critic}
 
 
 @dataclass
@@ -143,6 +155,8 @@ class TrackingEnvCfg:
   policy_corruption: bool = True           # the policy group's enable_corruption
   # per-episode logs of the reward, termination and command managers (reward_log, termination_log, command_log)
   episode_logs: bool = False
+  # clip, scale and history of the policy and critic groups (terms: obs_terms); the defaults leave both as computed
+  observations: ObservationsCfg = field(default_factory=ObservationsCfg)
 
   def __post_init__(self):
     self.check()
@@ -306,7 +320,9 @@ class TrackingFlatEnv:
     self.reward_stds = [float(getattr(rc, t + "_std")) for t in TRACKING_TERMS]
     self.term_thresholds = [getattr(tc, t) for t in TERMINATION_TERMS[1:]]
     self._push_r = None if cfg.push_velocity_range is None else torch.tensor(cfg.push_velocity_range, **f32)
-    self.nobs = 5 * self.nu + (15 if cfg.policy_state_estimation else 9)
+    self.obs_groups = Observations(cfg.observations, obs_terms(self.nu, len(BODY_NAMES), cfg.policy_state_estimation),
+                                   n, self.device)
+    self.nobs, self.nobs_critic = self.obs_groups.width("policy"), self.obs_groups.width("critic")  # elements per env
     self.episode_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
     self.finished_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
     self.term_flags = torch.zeros(n, len(TERMINATION_TERMS), **f32)
@@ -510,7 +526,9 @@ class TrackingFlatEnv:
     self._resample(all_, all_, self._rand(self.num_envs, 13 + self.nu))
     self.sim.forward()
     self._update_command()
-    return self.observations()
+    policy, critic = self.observations()
+    out = self.obs_groups.fill({"policy": policy, "critic": critic})
+    return out["policy"], out["critic"]
 
   def enable_cuda_graph(self) -> None:
     dev = torch.device(self.device)
@@ -551,7 +569,7 @@ class TrackingFlatEnv:
     self._reward = torch.zeros(n, **f32)
     self._term = torch.zeros(n, dtype=torch.bool, device=dev)
     self._trunc = torch.zeros(n, dtype=torch.bool, device=dev)
-    self._obs = torch.zeros(n, self.nobs, **f32)
+    self._obs = torch.zeros(n, 5 * nu + (15 if self.cfg.policy_state_estimation else 9), **f32)
     self._critic = torch.zeros(n, 5 * nu + 15 + 9 * nb, **f32)
     self._body_idx32 = self.robot.indexing.body_ids[self.body_idx].to(torch.int32).contiguous()
     self._ee_idx32 = self.ee_idx.to(torch.int32).contiguous()
@@ -610,6 +628,7 @@ class TrackingFlatEnv:
       ptr.update(logs)
     self._native_args = A
     self._keep = ptr
+    self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
 
   def _step_native(self, action: torch.Tensor, U: torch.Tensor):
     """Two fused kernels around the masked forward (csrc/b2_trackenv.cuh) instead of ~150 torch launches."""
@@ -628,7 +647,7 @@ class TrackingFlatEnv:
 
   def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
     """Everything after the sub-steps on the fused path: post1 (and the sampler's bins), the forward of the reset
-    envs, post2."""
+    envs, post2, and the observation groups' clip, scale and history (b2_obs_history, when configured)."""
     import ctypes
 
     if getattr(self, "_native_args", None) is None:
@@ -644,7 +663,8 @@ class TrackingFlatEnv:
       native.check(sim._lib.b2_trackenv_bins(sim._h, ctypes.byref(self._native_args), st))
     sim.forward(env_mask=self._done_buf)
     native.check(sim._lib.b2_trackenv_post2(sim._h, ctypes.byref(self._native_args), st))
-    return self._obs, self._reward, self._term, self._trunc, self._extras(self._critic)
+    out = self.obs_groups.run_native(sim, {"policy": self._obs, "critic": self._critic})
+    return out["policy"], self._reward, self._term, self._trunc, self._extras(out["critic"])
 
   def _step_torch(self, action: torch.Tensor, U: torch.Tensor):
     self.sim.data.ctrl[:] = self.default_joint_pos + self.action_scale * action  # JointPositionAction, use_default_offset
@@ -742,7 +762,8 @@ class TrackingFlatEnv:
       lo_t, hi_t = cfg.push_interval_s
       self.push_time_left.copy_(torch.where(push, P[:, 6] * (hi_t - lo_t) + lo_t, self.push_time_left))
     policy, critic = self.observations(U[:, 2 * S + 7:])
-    return policy, reward, terminated, truncated, self._extras(critic)
+    out = self.obs_groups.update({"policy": policy, "critic": critic}, terminated | truncated)
+    return out["policy"], reward, terminated, truncated, self._extras(out["critic"])
 
   def close(self):
     self.sim.close()

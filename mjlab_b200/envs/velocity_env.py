@@ -19,6 +19,7 @@ import numpy as np
 import torch
 
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
+from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
 
 
@@ -26,6 +27,12 @@ REWARD_TERMS = ("track_lin_vel_exp", "track_ang_vel_exp", "pose", "dof_pos_limit
                 "air_time", "feet_slide", "foot_clearance", "is_alive", "is_terminated", "joint_torques_l2",
                 "joint_acc_l2", "electrical_power_cost", "flat_orientation_l2")  # opt-in (VelocityRewardsCfg)
 NFIXED = 5
+# the terms of both observation groups, in frame order (velocity_env_cfg.py:86-131); elements per term
+OBS_TERMS = ("base_lin_vel", "base_ang_vel", "projected_gravity", "joint_pos", "joint_vel", "actions", "command")
+
+
+def obs_terms(nu: int) -> list[tuple[str, int]]:
+  return list(zip(OBS_TERMS, (3, 3, 3, nu, nu, nu, 3)))
 
 
 @dataclass
@@ -124,6 +131,8 @@ class VelocityEnvCfg:
   # per-joint widths of the posture reward (posture, envs/mdp/rewards.py:73-104): {joint regex: std}, every joint
   # matched by exactly one pattern and every pattern by some joint.  None: one width of 0.3 for every joint
   posture_std: dict | None = None
+  # clip, scale and history of the policy and critic groups (terms: OBS_TERMS); the defaults leave both as computed
+  observations: ObservationsCfg = field(default_factory=ObservationsCfg)
 
 
 def _float32(x) -> float:
@@ -271,6 +280,8 @@ class VelocityFlatEnv:
     self.push_time_left.copy_(self._rand(n) * (hi_t - lo_t) + lo_t)
     self._init_rewards()
     self._init_command(jnames)
+    self.obs_groups = Observations(cfg.observations, {g: obs_terms(self.nu) for g in ("policy", "critic")}, n, device)
+    self.nobs, self.nobs_critic = self.obs_groups.width("policy"), self.obs_groups.width("critic")  # elements per env
     if self.native_mdp:
       self._init_native()
     self._reset_all(curriculum=False)  # no episode has ended yet: the initial levels stand
@@ -415,13 +426,13 @@ class VelocityFlatEnv:
     from mjlab_b200.sim import native
 
     n, dev = self.num_envs, self.device
-    self.nobs = 9 + 3 * self.nu + 3
-    self._obs = torch.zeros(n, self.nobs, device=dev)
+    nframe = 9 + 3 * self.nu + 3
+    self._obs = torch.zeros(n, nframe, device=dev)
     self._reward = torch.zeros(n, device=dev)
     self._term = torch.zeros(n, dtype=torch.bool, device=dev)
     self._trunc = torch.zeros(n, dtype=torch.bool, device=dev)
     self._U = torch.zeros(n, 16 + 9 + 2 * self.nu, device=dev)
-    self._critic = torch.zeros(n, self.nobs, device=dev)
+    self._critic = torch.zeros(n, nframe, device=dev)
     self._action_in = torch.zeros(n, self.nu, device=dev)
     self._origins = self.env_origins.contiguous()
     a = native.B2VelEnvArgs()
@@ -481,6 +492,7 @@ class VelocityFlatEnv:
       setattr(a, name, t.data_ptr())
     a.metric_steps = self.metric_steps
     self._native_args = a
+    self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
     """reset_root_state_uniform + reset_joints_by_scale (envs/mdp/events.py:43-124) for masked envs."""
@@ -646,7 +658,8 @@ class VelocityFlatEnv:
     self._reset_where(all_, U)
     self.sim.forward()
     self._update_command(all_, U, metrics=False)
-    return self.observations()
+    frame = self.observations()
+    return self.obs_groups.fill({"policy": frame, "critic": frame})["policy"]
 
   def enable_cuda_graph(self) -> None:
     """Capture one whole env step (ctrl write, 4 sub-steps, MDP glue, masked reset + forward) in a
@@ -692,7 +705,8 @@ class VelocityFlatEnv:
     return self._mdp_native(self._action_in, self._U)
 
   def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
-    """Everything after the sub-steps on the fused path: b2_velenv_post, then the forward of the reset envs."""
+    """Everything after the sub-steps on the fused path: b2_velenv_post, then the forward of the reset envs and the
+    observation groups' clip, scale and history (b2_obs_history, when configured)."""
     import ctypes
 
     from mjlab_b200.sim import native
@@ -704,7 +718,8 @@ class VelocityFlatEnv:
       self._U.copy_(U)
     native.check(sim._lib.b2_velenv_post(sim._h, ctypes.byref(self._native_args), sim._stream()))
     sim.forward(env_mask=self._done_buf)
-    return self._obs, self._reward, self._term, self._trunc, {"critic": self._critic}
+    out = self.obs_groups.run_native(sim, {"policy": self._obs, "critic": self._critic})
+    return out["policy"], self._reward, self._term, self._trunc, {"critic": out["critic"]}
 
   def _step_torch(self, action: torch.Tensor):
     """Reference implementation of the same step in torch ops (also the checker of the fused kernels)."""
@@ -761,8 +776,8 @@ class VelocityFlatEnv:
     d.qvel[:, 0:2] = torch.where(push.unsqueeze(1), pv, d.qvel[:, 0:2])
     lo_t, hi_t = cfg.push_interval_s
     self.push_time_left.copy_(torch.where(push, U[:, 11] * (hi_t - lo_t) + lo_t, self.push_time_left))
-    obs = self.observations(U)
-    return obs, reward, terminated, truncated, {"critic": self.critic_obs}
+    out = self.obs_groups.update({"policy": self.observations(U), "critic": self.critic_obs}, terminated | truncated)
+    return out["policy"], reward, terminated, truncated, {"critic": out["critic"]}
 
   def close(self):
     self.sim.close()

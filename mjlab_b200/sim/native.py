@@ -103,6 +103,26 @@ class B2TrackEnvArgs(ctypes.Structure):
 TRACKENV_NREW, TRACKENV_NTERM, TRACKENV_NMETRIC = 9, 4, 10  # B2_TRACKENV_N*: log columns of B2TrackEnvArgs
 
 
+OBSHIST_NTERM, OBSHIST_NGROUP = 16, 2  # B2_OBSHIST_NTERM / B2_OBSHIST_NGROUP: terms per group, groups per launch
+
+
+class B2ObsHistTerm(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_int32) for n in ("src", "dim", "frames", "dst", "stride", "scale", "clip")]
+              + [(n, ctypes.c_float) for n in ("lo", "hi")])
+
+
+class B2ObsHistGroup(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_void_p) for n in ("frame", "out")]
+              + [(n, ctypes.c_int32) for n in ("frame_width", "out_width", "nterm")]
+              + [("term", B2ObsHistTerm * OBSHIST_NTERM)])
+
+
+class B2ObsHistArgs(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_void_p) for n in ("terminated", "truncated", "scale")]
+              + [(n, ctypes.c_int32) for n in ("nscale", "ngroup")]
+              + [("group", B2ObsHistGroup * OBSHIST_NGROUP)])
+
+
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
 
 
@@ -160,6 +180,7 @@ def bind(L: ctypes.CDLL) -> ctypes.CDLL:
     "b2_trackenv_post1": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_trackenv_post2": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_trackenv_bins": ([vp, P(B2TrackEnvArgs), vp], ci),
+    "b2_obs_history": ([vp, P(B2ObsHistArgs), vp], ci),
     "b2_stats": ([vp, vp, P(B2Stats)], ci),
     "b2_launch_count": ([vp], ctypes.c_int64),
     "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),
