@@ -349,6 +349,46 @@ typedef struct B2ObsHistArgs {
 } B2ObsHistArgs;
 int b2_obs_history(b2_sim* sim, const B2ObsHistArgs* args, void* cuda_stream);
 
+/* ---- reset and interval randomize_field events (the reference's EventManager.apply("reset") / apply("interval") /
+ * reset, managers/event_manager.py:76-167, with envs/mdp/events.py:212-397) ------------------------------------------
+ * One launch per env step, after the env's post kernel (b2_velenv_post, b2_trackenv_post1 / bins) and before the
+ * masked forward.  In env w the terms run in table order; a term fires when
+ *   mode RESET:    w's terminated or truncated byte is set (the reference's reset_buf);
+ *   mode INTERVAL: t = timers[k][w] (k: the term's rank among the interval terms) takes t -= step_dt; it fires when
+ *                  t < 1e-6, and t is then redrawn, t = lo + V[w][col + count] span.  Every step stores t; a reset
+ *                  does not redraw it (EventManager.reset redraws only the timers of class-based terms).
+ * When it fires, entry j of its count (element, axis) entries, e = elem[first + j] (first: the counts of the terms
+ * before it), draws x = lo + V[w][col + j] span (one fp32 product, then one fp32 sum); LOG_UNIFORM takes exp(x).  It
+ * then writes row[e.offset] = row + x (ADD), row x (SCALE) or x (ABS), where row is world w's row of model field
+ * `field`, the field's index in the library's model-field table (b2_field_name(sim, B2_MODEL, field)).  The field must
+ * be a float model field with a per-world copy (b2_expand_model_field) and every offset inside its row. */
+#define B2_EVENTS_NTERM 16   /* reset and interval terms per launch */
+enum { B2_EVENT_RESET = 0, B2_EVENT_INTERVAL = 1 };
+enum { B2_EVENT_ADD = 0, B2_EVENT_SCALE = 1, B2_EVENT_ABS = 2 };
+enum { B2_EVENT_UNIFORM = 0, B2_EVENT_LOG_UNIFORM = 1 };
+typedef struct B2EventTerm {
+  int32_t mode, operation, distribution;
+  int32_t field;                  /* index in the model-field table */
+  int32_t count;                  /* (element, axis) entries, >= 1 */
+  int32_t col;                    /* first V column: count draws, then (INTERVAL) the timer's redraw */
+  float interval_lo, interval_span; /* INTERVAL: the timer's draw lo + u span */
+} B2EventTerm;
+typedef struct B2EventElem {
+  int32_t offset;                 /* element index in the world's row of the field (element * width + axis) */
+  float lo, span;                 /* the draw lo + u span (LOG_UNIFORM: of the logarithm) */
+} B2EventElem;
+typedef struct B2EventArgs {
+  const unsigned char* terminated; /* [n] this env step's terminations */
+  const unsigned char* truncated;  /* [n] this env step's time-outs */
+  const float* V;                 /* [n][v_width] this env step's uniforms of the events */
+  float* timers;                  /* [ninterval][n] in/out: time left of each interval term */
+  const B2EventElem* elem;        /* [nelem] the terms' entries, term by term */
+  int32_t v_width, ninterval, nelem, nterm;
+  float step_dt;
+  B2EventTerm term[B2_EVENTS_NTERM];
+} B2EventArgs;
+int b2_events(b2_sim* sim, const B2EventArgs* args, void* cuda_stream);
+
 /* Diagnostics (synchronises `cuda_stream`). */
 int b2_stats(b2_sim* sim, void* cuda_stream, B2Stats* out);
 /* Number of kernels this library has launched for `sim` since creation. */

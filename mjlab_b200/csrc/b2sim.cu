@@ -16,6 +16,7 @@
 #include "b2_env.cuh"
 #include "b2_trackenv.cuh"
 #include "b2_obshist.cuh"
+#include "b2_events.cuh"
 
 static thread_local std::string g_err;
 static int fail(const std::string& msg) {
@@ -68,6 +69,7 @@ struct b2_sim {
   cudaStream_t side[2] = {nullptr, nullptr};  // b2_step_n's two env partitions
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
   size_t smem_bytes = 0;
+  std::vector<long long> events_checked;  // b2_events: the entry table last checked (address, size, fields, counts)
 };
 
 static int pad4(int n) { return (n + 3) & ~3; }
@@ -1228,6 +1230,73 @@ int b2_obs_history(b2_sim* s, const B2ObsHistArgs* args, void* stream) {
   for (int g = 0; g < args->ngroup; g++) total += (long long)s->nworld * args->group[g].frame_width;
   DeviceGuard guard(s->device);
   b2_obs_history_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(s->nworld, *args);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+static int events_check(b2_sim* s, const B2EventArgs* a, B2EventFields* F) {
+  if (!s || !a) return fail("b2_events: bad arguments");
+  if (!a->terminated || !a->truncated || !a->V || !a->elem || a->v_width < 1 || a->nterm < 1 ||
+      a->nterm > B2_EVENTS_NTERM || a->ninterval < 0 || a->nelem < 1 || !(a->step_dt > 0.0f))
+    return fail("b2_events: needs terminated, truncated, V (v_width >= 1), the entry table, "
+                "1 <= nterm <= B2_EVENTS_NTERM and step_dt > 0");
+  long long first = 0;
+  int ninterval = 0;
+  for (int t = 0; t < a->nterm; t++) {
+    const B2EventTerm& T = a->term[t];
+    if ((T.mode != B2_EVENT_RESET && T.mode != B2_EVENT_INTERVAL) ||
+        (T.operation != B2_EVENT_ADD && T.operation != B2_EVENT_SCALE && T.operation != B2_EVENT_ABS) ||
+        (T.distribution != B2_EVENT_UNIFORM && T.distribution != B2_EVENT_LOG_UNIFORM))
+      return fail("b2_events: term " + std::to_string(t) + " has an unknown mode, operation or distribution code");
+    if (T.field < 0 || T.field >= (int)s->model_fields.size() || !s->model_fields[T.field].farr)
+      return fail("b2_events: term " + std::to_string(t) + "'s field is not a float model field");
+    const Field& f = s->model_fields[T.field];
+    if (f.farr->stride == 0 && s->nworld > 1)
+      return fail("b2_events: field '" + f.name + "' is shared by every world; b2_expand_model_field it first");
+    const bool interval = T.mode == B2_EVENT_INTERVAL;
+    if (T.count < 1 || T.col < 0 || (long long)T.col + T.count + (interval ? 1 : 0) > a->v_width ||
+        first + T.count > a->nelem)
+      return fail("b2_events: term " + std::to_string(t) + " reads V columns outside the block or entries outside "
+                  "the table");
+    if (interval && !(T.interval_lo >= 0.0f && T.interval_span >= 0.0f && T.interval_lo + T.interval_span < INFINITY))
+      return fail("b2_events: term " + std::to_string(t) + " needs a finite interval with 0 <= lo and span >= 0");
+    F->row[t] = const_cast<float*>(f.farr->p);
+    F->stride[t] = f.farr->stride;
+    first += T.count;
+    ninterval += interval;
+  }
+  if (first != a->nelem) return fail("b2_events: the terms' counts do not add up to nelem");
+  if (ninterval > a->ninterval || (ninterval > 0 && !a->timers))
+    return fail("b2_events: the interval terms need their timers ([ninterval][n])");
+  // The entry table is device memory: it is read back and checked the first time this sim sees it with these fields
+  // and counts (a synchronising copy, so outside a stream capture), and taken as unchanged after that, so that the
+  // calls an env step captures read nothing back.
+  std::vector<long long> key = {(long long)(uintptr_t)a->elem, a->nelem};
+  for (int t = 0; t < a->nterm; t++) key.insert(key.end(), {a->term[t].field, a->term[t].count});
+  if (key == s->events_checked) return 0;
+  std::vector<B2EventElem> elem(a->nelem);
+  CUDA_OK(cudaMemcpy(elem.data(), a->elem, sizeof(B2EventElem) * elem.size(), cudaMemcpyDeviceToHost));
+  first = 0;
+  for (int t = 0; t < a->nterm; t++) {
+    const Field& f = s->model_fields[a->term[t].field];
+    for (int j = 0; j < a->term[t].count; j++) {
+      const B2EventElem& E = elem[first + j];
+      if (E.offset < 0 || E.offset >= f.farr->n)
+        return fail("b2_events: term " + std::to_string(t) + " writes element " + std::to_string(E.offset) +
+                    ", outside the row of '" + f.name + "' (" + std::to_string(f.farr->n) + " floats)");
+    }
+    first += a->term[t].count;
+  }
+  s->events_checked = key;
+  return 0;
+}
+int b2_events(b2_sim* s, const B2EventArgs* args, void* stream) {
+  B2EventFields F = {};
+  DeviceGuard guard(s ? s->device : 0);
+  if (events_check(s, args, &F)) return 1;
+  const long long threads = 32LL * s->nworld;
+  b2_events_kernel<<<(unsigned)((threads + 127) / 128), 128, 0, (cudaStream_t)stream>>>(s->nworld, *args, F);
   s->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -34,6 +34,7 @@ import torch.nn.functional as F
 
 from mjlab_b200.asset_zoo import g1, load_compiled
 from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply, quat_apply_inverse, quat_mul
+from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
 from mjlab_b200.envs.motion import MotionClip
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.envs.velocity_env import _resolve
@@ -157,6 +158,8 @@ class TrackingEnvCfg:
   episode_logs: bool = False
   # clip, scale and history of the policy and critic groups (terms: obs_terms); the defaults leave both as computed
   observations: ObservationsCfg = field(default_factory=ObservationsCfg)
+  # randomize_field events (envs/events.py), run after the task's startup randomisation (startup_events)
+  events: EventsCfg = field(default_factory=EventsCfg)
 
   def __post_init__(self):
     self.check()
@@ -164,6 +167,7 @@ class TrackingEnvCfg:
   def check(self) -> None:
     self.rewards.check()
     self.terminations.check()
+    self.events.check()
     _check_range6("pose_range", self.pose_range)
     _check_range6("velocity_range", self.velocity_range)
     if self.push_velocity_range is not None:
@@ -184,6 +188,15 @@ TRACKING_TASKS = {
   "Mjlab-Tracking-Flat-Unitree-G1-No-State-Estimation": dict(policy_state_estimation=False),
   "Mjlab-Tracking-Flat-Unitree-G1-No-State-Estimation-Play": dict(_PLAY, policy_state_estimation=False),
 }
+
+
+def startup_events(cfg: TrackingEnvCfg) -> tuple:
+  """The task's startup randomisation (tracking_env_cfg.py:162-198): the torso's COM offset, the joints' default
+  positions and the feet's friction (friction_range)."""
+  return (RandomizeFieldCfg("body_ipos", {0: (-0.025, 0.025), 1: (-0.05, 0.05), 2: (-0.05, 0.05)}, operation="add",
+                            names="torso_link"),
+          RandomizeFieldCfg("qpos0", (-0.01, 0.01), operation="add"),
+          RandomizeFieldCfg("geom_friction", tuple(cfg.friction_range), operation="abs", names=tuple(g1.FOOT_GEOMS)))
 
 
 def tracking_task_cfg(name: str, **overrides) -> TrackingEnvCfg:
@@ -259,15 +272,11 @@ class TrackingFlatEnv:
     self.env_origins = torch.stack(
       [(idx // cols - (cols - 1) / 2) * cfg.env_spacing, (idx % cols - (cols - 1) / 2) * cfg.env_spacing,
        torch.zeros(n, device=dev)], dim=1).float()
-    # ---- startup domain randomisation (tracking_env_cfg.py:162-198) -----------------------------------
-    self.sim.expand_model_fields(["body_ipos", "qpos0", "geom_friction"])
-    torso = ix.body_ids[ix.body_names.index("torso_link")].long()
-    rng = torch.tensor([[-0.025, 0.025], [-0.05, 0.05], [-0.05, 0.05]], **f32)
-    self.sim.model.body_ipos[:, torso] += self._rand(n, 3) * (rng[:, 1] - rng[:, 0]) + rng[:, 0]
-    self.sim.model.qpos0[:, ix.joint_q_adr.long()] += self._rand(n, self.nu) * 0.02 - 0.01
-    feet = torch.tensor([m.names["geom"].index(f"robot/{g}") for g in g1.FOOT_GEOMS], device=dev)
-    lo, hi = cfg.friction_range
-    self.sim.model.geom_friction[:, feet, 0] = self._rand(n, len(feet)) * (hi - lo) + lo
+    # ---- domain randomisation: the task's startup terms, then cfg.events; the fields they name get a per-world copy
+    self.events = Events(startup_events(cfg) + tuple(cfg.events.terms), ix, self.sim, n, self.step_dt, device)
+    self.sim.expand_model_fields(self.events.fields())
+    self.events.run_startup(self._rand)
+    self.events.draw_timers(self._rand)
     self.sim.data.qpos[:] = self.default_qpos
     self.sim.data.qvel[:] = 0.0
     self.sim.forward()
@@ -524,6 +533,7 @@ class TrackingFlatEnv:
       t.zero_()
     all_ = torch.ones(self.num_envs, dtype=torch.bool, device=self.device)
     self._resample(all_, all_, self._rand(self.num_envs, 13 + self.nu))
+    self.events.reset_all(self._rand)
     self.sim.forward()
     self._update_command()
     policy, critic = self.observations()
@@ -555,6 +565,7 @@ class TrackingFlatEnv:
   def _step_impl(self, action: torch.Tensor):
     n = self.num_envs
     U = self._rand(n, 48 + 4 * self.nu)  # B2_TRACKENV_NU: every random number of this env step (include/b2sim.h)
+    self.events.draw(self._rand)         # (and those of the reset and interval events, when there are any)
     if self.native_mdp:
       return self._step_native(action, U)
     return self._step_torch(action, U)
@@ -629,6 +640,7 @@ class TrackingFlatEnv:
     self._native_args = A
     self._keep = ptr
     self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
+    self.events.bind(self._term, self._trunc)
 
   def _step_native(self, action: torch.Tensor, U: torch.Tensor):
     """Two fused kernels around the masked forward (csrc/b2_trackenv.cuh) instead of ~150 torch launches."""
@@ -646,8 +658,9 @@ class TrackingFlatEnv:
     return self._mdp_native(self._act, self._U)
 
   def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
-    """Everything after the sub-steps on the fused path: post1 (and the sampler's bins), the forward of the reset
-    envs, post2, and the observation groups' clip, scale and history (b2_obs_history, when configured)."""
+    """Everything after the sub-steps on the fused path: post1 (and the sampler's bins), the reset and interval
+    events (b2_events, when configured), the forward of the reset envs, post2, and the observation groups' clip, scale
+    and history (b2_obs_history, when configured)."""
     import ctypes
 
     if getattr(self, "_native_args", None) is None:
@@ -661,6 +674,7 @@ class TrackingFlatEnv:
     native.check(sim._lib.b2_trackenv_post1(sim._h, ctypes.byref(self._native_args), st))
     if self.start_mode == native.START_ADAPTIVE:
       native.check(sim._lib.b2_trackenv_bins(sim._h, ctypes.byref(self._native_args), st))
+    self.events.run_native(sim)
     sim.forward(env_mask=self._done_buf)
     native.check(sim._lib.b2_trackenv_post2(sim._h, ctypes.byref(self._native_args), st))
     out = self.obs_groups.run_native(sim, {"policy": self._obs, "critic": self._critic})
@@ -743,6 +757,7 @@ class TrackingFlatEnv:
     self._resample(ended, ended, U[:, S:2 * S])
     if self.start_mode == native.START_ADAPTIVE:
       self._sampler_step()
+    self.events.step_torch(terminated, truncated)  # reset, then interval events (before the forward, as b2_events)
     self._done_buf.copy_(done | ended)
     self.sim.forward(env_mask=self._done_buf)
     # a done env's motion errors: its reset state against the frame before the clip stepped and the stale targets

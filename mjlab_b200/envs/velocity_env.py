@@ -19,6 +19,8 @@ import numpy as np
 import torch
 
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
+from mjlab_b200.entity_data import EntityIndexing
+from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
 
@@ -133,6 +135,8 @@ class VelocityEnvCfg:
   posture_std: dict | None = None
   # clip, scale and history of the policy and critic groups (terms: OBS_TERMS); the defaults leave both as computed
   observations: ObservationsCfg = field(default_factory=ObservationsCfg)
+  # randomize_field events (envs/events.py), run after the startup foot friction of friction_range
+  events: EventsCfg = field(default_factory=EventsCfg)
 
 
 def _float32(x) -> float:
@@ -255,14 +259,15 @@ class VelocityFlatEnv:
       self.move_up_dist = 0.5 * float(cfg.terrain_size[0])
       # the mean level terrain_levels_vel returns for logging, kept on the device (updated by the curriculum)
       self.terrain_level_mean = self.terrain_levels.float().mean()
-    # startup domain randomisation: foot friction (events.py:212-265 'abs' on geom_friction[:, feet, 0])
-    self.sim.expand_model_fields(["geom_friction"])
-    foot_ids = torch.tensor(
-      [m.names["geom"].index(f"robot/{g}") for g in zoo.FOOT_GEOMS], device=dev, dtype=torch.long
-    )
-    lo, hi = cfg.friction_range
-    mu = torch.rand((n, len(foot_ids)), generator=self.gen, device=dev) * (hi - lo) + lo
-    self.sim.model.geom_friction[:, foot_ids, 0] = mu
+    # domain randomisation: the task's startup foot friction (velocity_env_cfg.py:162-172), then cfg.events; the
+    # fields they name get a per-world copy first
+    cfg.events.check()
+    feet = RandomizeFieldCfg("geom_friction", tuple(cfg.friction_range), operation="abs", names=tuple(zoo.FOOT_GEOMS))
+    self.events = Events((feet,) + tuple(cfg.events.terms), EntityIndexing.from_model(m, "robot", device), self.sim,
+                         n, self.step_dt, device)
+    self.sim.expand_model_fields(self.events.fields())
+    self.events.run_startup(self._rand)
+    self.events.draw_timers(self._rand)
     self.episode_length_buf = torch.zeros(n, dtype=torch.int32, device=dev)
     self.last_action = torch.zeros(n, self.nu, **f32)
     self.command = torch.zeros(n, 3, **f32)
@@ -493,6 +498,7 @@ class VelocityFlatEnv:
     a.metric_steps = self.metric_steps
     self._native_args = a
     self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
+    self.events.bind(self._term, self._trunc)
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
     """reset_root_state_uniform + reset_joints_by_scale (envs/mdp/events.py:43-124) for masked envs."""
@@ -656,6 +662,7 @@ class VelocityFlatEnv:
     if curriculum:
       self._terrain_curriculum(all_, U)
     self._reset_where(all_, U)
+    self.events.reset_all(self._rand)
     self.sim.forward()
     self._update_command(all_, U, metrics=False)
     frame = self.observations()
@@ -698,6 +705,7 @@ class VelocityFlatEnv:
     sim = self.sim
     self._action_in.copy_(action)
     self._U.copy_(self._draw())
+    self.events.draw(self._rand)
     native.check(sim._lib.b2_velenv_pre(
       sim._h, ctypes.c_void_p(self._action_in.data_ptr()), ctypes.c_void_p(self.default_joint_pos.data_ptr()),
       ctypes.c_void_p(self.action_scale.data_ptr()), sim._stream()))
@@ -705,8 +713,9 @@ class VelocityFlatEnv:
     return self._mdp_native(self._action_in, self._U)
 
   def _mdp_native(self, action: torch.Tensor, U: torch.Tensor):
-    """Everything after the sub-steps on the fused path: b2_velenv_post, then the forward of the reset envs and the
-    observation groups' clip, scale and history (b2_obs_history, when configured)."""
+    """Everything after the sub-steps on the fused path: b2_velenv_post, the reset and interval events (b2_events,
+    when configured), then the forward of the reset envs and the observation groups' clip, scale and history
+    (b2_obs_history, when configured)."""
     import ctypes
 
     from mjlab_b200.sim import native
@@ -717,6 +726,7 @@ class VelocityFlatEnv:
     if U is not self._U:
       self._U.copy_(U)
     native.check(sim._lib.b2_velenv_post(sim._h, ctypes.byref(self._native_args), sim._stream()))
+    self.events.run_native(sim)
     sim.forward(env_mask=self._done_buf)
     out = self.obs_groups.run_native(sim, {"policy": self._obs, "critic": self._critic})
     return out["policy"], self._reward, self._term, self._trunc, {"critic": out["critic"]}
@@ -724,6 +734,7 @@ class VelocityFlatEnv:
   def _step_torch(self, action: torch.Tensor):
     """Reference implementation of the same step in torch ops (also the checker of the fused kernels)."""
     U = self._draw()
+    self.events.draw(self._rand)
     # JointPositionAction: target = default + scale * action (joint_actions.py:85-103)
     self.sim.data.ctrl[:] = self.default_joint_pos + self.action_scale * action
     self.sim.step_n(self.cfg.decimation)
@@ -765,6 +776,7 @@ class VelocityFlatEnv:
     if self.terrain_curriculum:
       self._terrain_curriculum(done, U)
     self._reset_where(done, U)
+    self.events.step_torch(terminated, truncated)  # reset, then interval events (before the forward, as b2_events)
     self._done_buf.copy_(done)
     self.sim.forward(env_mask=self._done_buf)  # only the reset envs need new derived quantities here
     self._update_command(done, U)

@@ -123,6 +123,26 @@ class B2ObsHistArgs(ctypes.Structure):
               + [("group", B2ObsHistGroup * OBSHIST_NGROUP)])
 
 
+EVENTS_NTERM = 16  # B2_EVENTS_NTERM: reset and interval terms per b2_events launch
+EVENT_RESET, EVENT_INTERVAL = 0, 1  # B2EventTerm.mode (B2_EVENT_* of include/b2sim.h); operation and distribution are
+# the indices of events.OPERATIONS ("add", "scale", "abs") and events.DISTRIBUTIONS ("uniform", "log_uniform")
+
+
+class B2EventTerm(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_int32) for n in ("mode", "operation", "distribution", "field", "count", "col")]
+              + [(n, ctypes.c_float) for n in ("interval_lo", "interval_span")])
+
+
+class B2EventElem(ctypes.Structure):
+  _fields_ = [("offset", ctypes.c_int32), ("lo", ctypes.c_float), ("span", ctypes.c_float)]
+
+
+class B2EventArgs(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_void_p) for n in ("terminated", "truncated", "V", "timers", "elem")]
+              + [(n, ctypes.c_int32) for n in ("v_width", "ninterval", "nelem", "nterm")]
+              + [("step_dt", ctypes.c_float), ("term", B2EventTerm * EVENTS_NTERM)])
+
+
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
 
 
@@ -181,6 +201,7 @@ def bind(L: ctypes.CDLL) -> ctypes.CDLL:
     "b2_trackenv_post2": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_trackenv_bins": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_obs_history": ([vp, P(B2ObsHistArgs), vp], ci),
+    "b2_events": ([vp, P(B2EventArgs), vp], ci),
     "b2_stats": ([vp, vp, P(B2Stats)], ci),
     "b2_launch_count": ([vp], ctypes.c_int64),
     "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),
