@@ -321,9 +321,26 @@ int b2_trackenv_bins(b2_sim* sim, const B2TrackEnvArgs* args, void* cuda_stream)
  *   every frame moves one slot older and v is written into the newest; an env whose terminated or truncated byte is
  *   set (the reference's reset_buf) gets v in every slot.
  * The terms tile the frame row in order (src of term 0 is 0, each next src is the previous src + dim, the last ends at
- * frame_width), and their frames tile the out row: every column of out is written by exactly one element. */
+ * frame_width), and their frames tile the out row: every column of out is written by exactly one element.
+ *
+ * Noise (the block appended at the end of B2ObsHistArgs; ObservationTermCfg.noise, utils/noise/).  A group whose
+ * noise[g].source is set reads v from source[w][col + j] (the term's noise-free values) instead of frame, and before
+ * the clip, for a term with a bias code (NoiseModelWithAdditiveBias):
+ *   when w's terminated or truncated byte is set, bias[w][src + j] = redraw(bias[w][src + j]) and is stored;
+ *   v = noise(v) + bias[w][src + j]   (a term without a bias: v = noise(v); with neither code: v as loaded).
+ * A noise of class c, operation op, parameter rows p0, p1 (param[p0 + j], param[p1 + j]) and draw r is, in IEEE fp32
+ * with one rounding per operation (no contraction, subnormals kept):
+ *   CONSTANT: x = p0 (bias);  UNIFORM: x = r p1 + p0 (r = W[w][draw + j], p1 the span, p0 n_min);
+ *   GAUSSIAN: x = r p1 + p0 (r = N[w][draw + j], p1 std, p0 mean);
+ *   ADD: v + x;  SCALE: v x;  ABS: x (0 + x for CONSTANT).
+ * The bias redraw is the same with the bias fields, applied to the old bias; with bias_shared = 1 every element draws
+ * from column bias_draw (so the term's copies of a shared bias stay equal).  A term with a code needs the group's
+ * source (and bias row for a bias code), its columns inside the source row, its parameter rows inside param, its draws
+ * inside W or N, and W / N themselves. */
 #define B2_OBSHIST_NTERM 16  /* terms per group */
 #define B2_OBSHIST_NGROUP 2  /* groups per launch (policy, critic) */
+enum { B2_NOISE_NONE = 0, B2_NOISE_CONSTANT = 1, B2_NOISE_UNIFORM = 2, B2_NOISE_GAUSSIAN = 3 };
+enum { B2_NOISE_ADD = 0, B2_NOISE_SCALE = 1, B2_NOISE_ABS = 2 };
 typedef struct B2ObsHistTerm {
   int32_t src;                    /* first column of the term in the frame row */
   int32_t dim;                    /* elements of one frame of the term, >= 1 */
@@ -340,12 +357,33 @@ typedef struct B2ObsHistGroup {
   int32_t frame_width, out_width, nterm;
   B2ObsHistTerm term[B2_OBSHIST_NTERM];
 } B2ObsHistGroup;
+typedef struct B2ObsNoiseTerm {
+  int32_t col;                    /* first column of the term in the group's source row */
+  int32_t noise, noise_op;        /* B2_NOISE_* class (NONE: no noise) and operation of the per-step noise */
+  int32_t noise_p0, noise_p1;     /* offsets of its parameter rows in param (p1 unused by CONSTANT) */
+  int32_t noise_draw;             /* first column of its draws in W (UNIFORM) or N (GAUSSIAN) */
+  int32_t bias, bias_op;          /* class (NONE: no bias) and operation of the bias redraw */
+  int32_t bias_p0, bias_p1, bias_draw;
+  int32_t bias_shared;            /* 1: one draw per term; 0: one per element */
+} B2ObsNoiseTerm;
+typedef struct B2ObsNoiseGroup {
+  const float* source;            /* [n][source_width] noise-free term values; null: the group reads frame, no noise */
+  float* bias;                    /* [n][frame_width] in/out: the bias of element e at column e */
+  int32_t source_width, pad_;
+  B2ObsNoiseTerm term[B2_OBSHIST_NTERM];
+} B2ObsNoiseGroup;
 typedef struct B2ObsHistArgs {
   const unsigned char* terminated; /* [n] this env step's terminations */
   const unsigned char* truncated;  /* [n] this env step's time-outs */
   const float* scale;             /* [nscale] per-element factors of the scaled terms; may be null when nscale = 0 */
   int32_t nscale, ngroup;         /* 1 <= ngroup <= B2_OBSHIST_NGROUP */
   B2ObsHistGroup group[B2_OBSHIST_NGROUP];
+  /* noise (all zero: none) */
+  const float* W;                 /* [n][nW] this env step's uniforms of the noise; may be null when no term draws */
+  const float* N;                 /* [n][nN] this env step's standard normals of the noise */
+  const float* param;             /* [nparam] the terms' per-element parameter rows */
+  int32_t nW, nN, nparam;
+  B2ObsNoiseGroup noise[B2_OBSHIST_NGROUP];  /* noise[g] belongs to group[g] */
 } B2ObsHistArgs;
 int b2_obs_history(b2_sim* sim, const B2ObsHistArgs* args, void* cuda_stream);
 

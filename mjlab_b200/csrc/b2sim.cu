@@ -1190,6 +1190,50 @@ int b2_trackenv_bins(b2_sim* s, const B2TrackEnvArgs* args, void* stream) {
   return 0;
 }
 
+// The noise block of group g (include/b2sim.h): known codes, and every column, parameter and draw a term reads inside
+// its row.
+static int obsnoise_check(const B2ObsHistArgs* a, int g) {
+  const B2ObsHistGroup& G = a->group[g];
+  const B2ObsNoiseGroup& Z = a->noise[g];
+  if (a->nW < 0 || a->nN < 0 || a->nparam < 0)
+    return fail("b2_obs_history: nW, nN and nparam must be >= 0");
+  // one noise class: its parameter rows inside param, its `count` draws from column `draw` inside W or N
+  auto noise_ok = [&](int cls, int op, int p0, int p1, int draw, int dim, int count, const char** why) {
+    if (cls < B2_NOISE_NONE || cls > B2_NOISE_GAUSSIAN || op < B2_NOISE_ADD || op > B2_NOISE_ABS)
+      return *why = "an unknown noise class or operation", false;
+    if (cls == B2_NOISE_NONE) return true;
+    auto in_param = [&](int p) { return a->param && p >= 0 && (long long)p + dim <= a->nparam; };
+    if (!in_param(p0) || (cls != B2_NOISE_CONSTANT && !in_param(p1)))
+      return *why = "a parameter row outside param (or no param)", false;
+    if (cls == B2_NOISE_CONSTANT) return true;
+    const float* row = cls == B2_NOISE_UNIFORM ? a->W : a->N;
+    const int width = cls == B2_NOISE_UNIFORM ? a->nW : a->nN;
+    if (!row || draw < 0 || (long long)draw + count > width)
+      return *why = "draws outside W or N (or no W or N)", false;
+    return true;
+  };
+  for (int t = 0; t < G.nterm; t++) {
+    const B2ObsNoiseTerm& M = Z.term[t];
+    const int dim = G.term[t].dim;
+    const char* why = nullptr;
+    if (!noise_ok(M.noise, M.noise_op, M.noise_p0, M.noise_p1, M.noise_draw, dim, dim, &why) ||
+        (M.bias_shared != 0 && M.bias_shared != 1 && (why = "bias_shared must be 0 or 1")) ||
+        !noise_ok(M.bias, M.bias_op, M.bias_p0, M.bias_p1, M.bias_draw, dim, M.bias_shared ? 1 : dim, &why))
+      return fail(std::string("b2_obs_history: noise of a term: ") + why);
+    if (M.noise == B2_NOISE_NONE && M.bias == B2_NOISE_NONE) {
+      if (Z.source && (M.col < 0 || (long long)M.col + dim > Z.source_width))
+        return fail("b2_obs_history: noise of a term: its source columns lie outside the source row");
+      continue;
+    }
+    if (!Z.source) return fail("b2_obs_history: noise of a term: the group has no source row");
+    if (M.col < 0 || (long long)M.col + dim > Z.source_width)
+      return fail("b2_obs_history: noise of a term: its source columns lie outside the source row");
+    if (M.bias != B2_NOISE_NONE && !Z.bias) return fail("b2_obs_history: noise of a term: a bias needs the bias row");
+  }
+  if (Z.source && Z.source_width < 1) return fail("b2_obs_history: a source row needs source_width >= 1");
+  return 0;
+}
+
 static int obshist_check(b2_sim* s, const B2ObsHistArgs* a) {
   if (!s || !a) return fail("b2_obs_history: bad arguments");
   if (!a->terminated || !a->truncated || a->ngroup < 1 || a->ngroup > B2_OBSHIST_NGROUP || a->nscale < 0 ||
@@ -1221,6 +1265,7 @@ static int obshist_check(b2_sim* s, const B2ObsHistArgs* a) {
     }
     if (next != G.frame_width || covered != G.out_width)
       return fail("b2_obs_history: the terms' sizes do not add up to frame_width and out_width");
+    if (obsnoise_check(a, g)) return 1;
   }
   return 0;
 }

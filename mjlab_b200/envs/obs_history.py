@@ -19,6 +19,12 @@ history with the frame it computes.
 The output tensor is the history: the fused path's ``b2_obs_history`` kernel (``csrc/b2_obshist.cuh``) and the torch
 path below both update it in place.  A group left at its defaults is not processed at all: the env returns its frame,
 as it did before this existed.
+
+Noise (``envs/noise.py``).  A group is noise-configured when its ``noise`` dict is not empty or its
+``enable_corruption`` is set.  Such a group does not take the env's frame (whose built-in noise stays as it was for the
+groups that are not): each term reads its noise-free values from the env's critic frame, gets its effective noise (the
+task's default, replaced by a ``noise`` entry, none when the group's corruption is off), then the clip, scale and
+history above.  A group that is not noise-configured is untouched: same outputs, launches and draws.
 """
 
 from __future__ import annotations
@@ -30,6 +36,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import torch
 
+from mjlab_b200.envs import noise as nz
 from mjlab_b200.sim import native
 
 _F32_MAX = float(np.finfo(np.float32).max)
@@ -59,6 +66,9 @@ class ObsGroupCfg:
   term_history: dict = field(default_factory=dict)  # {term: history length}; 0: no history
   clip: dict = field(default_factory=dict)          # {term: (lo, hi)}
   scale: dict = field(default_factory=dict)         # {term: factor, or one factor per element of the term}
+  # {term: NoiseCfg | NoiseModelCfg | None} (envs/noise.py): replaces the task's default noise of the term; None: none
+  noise: dict = field(default_factory=dict)
+  enable_corruption: bool | None = None  # None: the task's setting for the group; False drops every term's noise
 
   def __post_init__(self):
     self.check()
@@ -76,7 +86,7 @@ class ObsGroupCfg:
       raise ValueError(f"{group}: history_length must be an integer >= 0 or None, not {self.history_length!r}")
     if not isinstance(self.flatten_history_dim, (bool, np.bool_)):
       raise ValueError(f"{group}: flatten_history_dim must be a bool, not {self.flatten_history_dim!r}")
-    for k in ("term_history", "clip", "scale"):
+    for k in ("term_history", "clip", "scale", "noise"):
       if not isinstance(getattr(self, k), dict):
         raise ValueError(f"{group}: {k} must be a dict keyed by term name")
     for t, h in self.term_history.items():
@@ -93,9 +103,13 @@ class ObsGroupCfg:
       vals = list(s) if isinstance(s, (tuple, list)) else [s]
       if not vals or not all(_finite32(v) for v in vals):
         raise ValueError(f"{group}: scale[{t!r}] = {s!r} must be a finite number or a tuple of finite numbers")
+    if self.enable_corruption is not None and not isinstance(self.enable_corruption, (bool, np.bool_)):
+      raise ValueError(f"{group}: enable_corruption must be a bool or None, not {self.enable_corruption!r}")
+    for t, c in self.noise.items():
+      nz.check_term_noise(c, terms[t] if terms is not None and t in terms else None, f"{group}: noise[{t!r}]")
     if terms is None:
       return
-    for k in ("term_history", "clip", "scale"):
+    for k in ("term_history", "clip", "scale", "noise"):
       unknown = [t for t in getattr(self, k) if t not in terms]
       if unknown:
         raise ValueError(f"{group}: {k} names unknown terms {unknown}; the group's terms are {list(terms)}")
@@ -126,16 +140,20 @@ class _Term:
   clip: tuple | None          # fp32 bounds
   scale: torch.Tensor | None  # [dim] fp32 factors
   scale_at: int               # offset in the env's scale row, -1: none
+  col: int = 0                # first column in the noise source row (noise-configured groups)
+  noise: nz.TermNoise | None = None  # effective noise
 
 
 class ObsGroup:
   """One group resolved against the env's terms: the layout of its output and the history buffer."""
 
   def __init__(self, cfg: ObsGroupCfg, group: str, terms: list[tuple[str, int]], num_envs: int, device,
-               scale_at: int = 0):
+               scale_at: int = 0, task_noise: nz.TaskNoise | None = None):
     cfg.check(dict(terms), group)
     H = cfg.lengths([t for t, _ in terms])
-    self.active = any(h > 0 for h in H) or bool(cfg.clip) or bool(cfg.scale)
+    # noise-configured: read the noise-free source row and apply the effective noise (module docstring)
+    self.noisy = bool(cfg.noise) or cfg.enable_corruption is not None
+    self.active = any(h > 0 for h in H) or bool(cfg.clip) or bool(cfg.scale) or self.noisy
     self.flatten = bool(cfg.flatten_history_dim)
     self.num_envs, self.frame_width = num_envs, sum(d for _, d in terms)
     dev = torch.device(device)
@@ -157,6 +175,27 @@ class ObsGroup:
       self.terms.append(t)
       src += dim
     self.scale_end = scale_at
+    self.bias = None  # [n, frame_width] the bias models' state, element e at column e
+    if self.noisy:
+      source = task_noise.source if task_noise is not None else terms
+      cols, c = {}, 0
+      for name, dim in source:
+        cols[name], c = c, c + dim
+      self.source_width = c
+      on = cfg.enable_corruption
+      if on is None:
+        on = bool(task_noise.corruption.get(group, False)) if task_noise is not None else False
+      defaults = task_noise.defaults.get(group, {}) if task_noise is not None else {}
+      for t in self.terms:
+        if t.name not in cols or dict(source)[t.name] != t.dim:
+          raise ValueError(f"{group}: the noise source row has no term {t.name!r} of {t.dim} elements")
+        t.col = cols[t.name]
+        eff = cfg.noise[t.name] if t.name in cfg.noise else defaults.get(t.name)
+        if on and eff is not None:
+          nz.check_term_noise(eff, t.dim, f"{group}: noise of {t.name!r}")
+          t.noise = nz.TermNoise(eff, t.dim, dev)
+      if any(t.noise is not None and t.noise.bias is not None for t in self.terms):
+        self.bias = torch.zeros(num_envs, self.frame_width, dtype=torch.float32, device=dev)
     self.shape = (num_envs, dst) if self.flatten else (num_envs, H[0], self.frame_width)
     self.width = int(np.prod(self.shape[1:]))  # elements per env
     self.out = torch.zeros(num_envs, self.width, dtype=torch.float32, device=dev) if self.active else None
@@ -170,12 +209,38 @@ class ObsGroup:
       return self.out[:, t.dst:t.dst + max(t.frames, 1) * t.dim].unflatten(1, (max(t.frames, 1), t.dim))
     return self.out.view(self.shape)[:, :, t.src:t.src + t.dim]
 
-  def update(self, frame: torch.Tensor, reset: torch.Tensor) -> torch.Tensor:
-    """The torch path: clip, scale and append `frame` [n, frame_width]; `reset` [n] bool backfills.  Returns a fresh
-    copy of the output."""
-    r = reset.view(-1, 1, 1)
+  def _bias(self, t: _Term) -> torch.Tensor:
+    return self.bias[:, t.src:t.src + t.dim]
+
+  def redraw_bias(self, mask: torch.Tensor | None, W, N, first: bool = False, shape: bool = False) -> None:
+    """Redraw the bias of every bias model in the envs of `mask` (None: all) from the draws W, N.  `first`: the
+    reference's first reset(all), when every bias is still (n, 1) and draws one column; `shape`: the first compute's
+    reshape of a per-component bias, which draws again per element (noise_model.py _initialize_bias_shape)."""
     for t in self.terms:
-      v = frame[:, t.src:t.src + t.dim]
+      d = t.noise.bias if t.noise is not None else None
+      if d is None or (shape and t.noise.shared):
+        continue
+      b = self._bias(t)
+      new = d.apply(b, _cols(d, W, N, 1 if first else None))
+      b.copy_(new if mask is None else torch.where(mask.view(-1, 1), new, b))
+
+  def update(self, frame: torch.Tensor, reset: torch.Tensor, source: torch.Tensor | None = None, W=None, N=None,
+             redraw: bool = True) -> torch.Tensor:
+    """The torch path: clip, scale and append `frame` [n, frame_width]; `reset` [n] bool backfills.  A
+    noise-configured group reads `source` instead and first redraws the biases of the reset envs (unless not
+    `redraw`) and adds the noise, from this step's draws W, N.  Returns a fresh copy of the output."""
+    r = reset.view(-1, 1, 1)
+    if self.noisy and redraw and self.bias is not None:
+      self.redraw_bias(reset, W, N)
+    for t in self.terms:
+      if self.noisy:
+        v = source[:, t.col:t.col + t.dim]
+        if t.noise is not None:
+          v = t.noise.noise.apply(v, _cols(t.noise.noise, W, N))
+          if t.noise.bias is not None:
+            v = v + self._bias(t)
+      else:
+        v = frame[:, t.src:t.src + t.dim]
       if t.clip is not None:
         v = v.clamp(t.clip[0], t.clip[1])
       if t.scale is not None:
@@ -197,33 +262,117 @@ class ObsGroup:
       T.clip = t.clip is not None
       T.lo, T.hi = t.clip if t.clip is not None else (0.0, 0.0)
 
+  def native_noise(self, Z: native.B2ObsNoiseGroup, source: torch.Tensor) -> None:
+    assert source.is_contiguous() and source.shape == (self.num_envs, self.source_width)
+    Z.source, Z.source_width = source.data_ptr(), self.source_width
+    if self.bias is not None:
+      Z.bias = self.bias.data_ptr()
+    for k, t in enumerate(self.terms):
+      M = Z.term[k]
+      M.col = t.col
+      if t.noise is None:
+        continue
+      d = t.noise.noise
+      M.noise, M.noise_op, M.noise_p0, M.noise_p1, M.noise_draw = d.kind, d.op, d.p0_at, d.p1_at, d.col
+      if t.noise.bias is not None:
+        d = t.noise.bias
+        M.bias, M.bias_op, M.bias_p0, M.bias_p1, M.bias_draw = d.kind, d.op, d.p0_at, d.p1_at, d.col
+        M.bias_shared = int(t.noise.shared)
+
+
+def _cols(d: nz.Draw, W, N, count: int | None = None):
+  """The draws of `d` (its first `count` columns; all by default), None for a constant."""
+  if d.kind == nz.CONSTANT:
+    return None
+  block = W if d.kind == nz.UNIFORM else N
+  return block[:, d.col:d.col + (d.ndraw if count is None else count)]
+
 
 class Observations:
   """The env's policy and critic groups: their outputs on both paths and the fused path's argument block."""
 
-  def __init__(self, cfg: ObservationsCfg, terms: dict, num_envs: int, device):
-    """`terms`: {group: [(term name, elements), ...]} in the order of the group's frame."""
+  def __init__(self, cfg: ObservationsCfg, terms: dict, num_envs: int, device, task_noise: nz.TaskNoise | None = None):
+    """`terms`: {group: [(term name, elements), ...]} in the order of the group's frame; `task_noise`: the task's
+    default noise and its noise-free source row (without it a noise-configured group reads its own frame and has no
+    default noise)."""
     self.groups, at = {}, 0
     for g in GROUPS:
-      self.groups[g] = ObsGroup(getattr(cfg, g), g, terms[g], num_envs, device, scale_at=at)
+      self.groups[g] = ObsGroup(getattr(cfg, g), g, terms[g], num_envs, device, scale_at=at, task_noise=task_noise)
       at = self.groups[g].scale_end
     scales = [t.scale for grp in self.groups.values() for t in grp.terms if t.scale is not None]
     self.scale_row = torch.cat(scales) if scales else None
     self.active = [g for g in GROUPS if self.groups[g].active]
     self._args = None
+    self._layout_noise(num_envs, device)
+
+  def _layout_noise(self, n: int, device) -> None:
+    """Columns of W and N and offsets in the parameter row of every term's noise, group by group, term by term: a
+    term's per-step draws, then its bias redraw."""
+    both = [t.name for g in GROUPS for t in self.groups[g].terms if t.noise is not None and t.noise.bias is not None]
+    if len(both) != len(set(both)):
+      raise ValueError("a bias model on the same term in both groups is not supported (the reference keys a bias "
+                       "model's state by term name, so both groups would share one)")
+    width, params, at = {"W": 0, "N": 0}, [], 0
+    for g in GROUPS:
+      for t in self.groups[g].terms:
+        if t.noise is None:
+          continue
+        for d in (t.noise.noise, t.noise.bias):
+          if d is None:
+            continue
+          if d.ndraw:
+            d.col, width[d.block] = width[d.block], width[d.block] + d.ndraw
+          for k, p in (("p0_at", d.p0), ("p1_at", d.p1)):
+            if p is not None:
+              setattr(d, k, at)
+              params.append(p)
+              at += p.numel()
+    self.nW, self.nN = width["W"], width["N"]
+    dev = torch.device(device)
+    self.W = torch.zeros(n, self.nW, dtype=torch.float32, device=dev) if self.nW else None
+    self.N = torch.zeros(n, self.nN, dtype=torch.float32, device=dev) if self.nN else None
+    self.param_row = torch.cat(params).contiguous() if params else None
+    self.noisy = [g for g in GROUPS if self.groups[g].noisy]
+    self._shaped = False  # whether the first reset reshaped the per-component biases
+
+  def draw(self, rand, randn) -> None:
+    """This step's blocks W (rand) and N (randn), when a term draws (the env calls it right after the events')."""
+    if self.W is not None:
+      self.W.copy_(rand(*self.W.shape))
+    if self.N is not None:
+      self.N.copy_(randn(*self.N.shape))
 
   def width(self, g: str) -> int:
     """Elements per env of group g's output."""
     return self.groups[g].width
 
-  def update(self, frames: dict, reset: torch.Tensor) -> dict:
-    """The torch path: each group's output from its frame (the frame itself for a group at its defaults)."""
-    return {g: self.groups[g].update(frames[g], reset) if self.groups[g].active else frames[g] for g in GROUPS}
+  def update(self, frames: dict, reset: torch.Tensor, redraw: bool = True) -> dict:
+    """The torch path: each group's output from its frame (the frame itself for a group at its defaults); a
+    noise-configured group reads the critic frame, the noise-free source, with this step's W and N."""
+    return {g: self.groups[g].update(frames[g], reset, frames["critic"], self.W, self.N, redraw)
+            if self.groups[g].active else frames[g] for g in GROUPS}
 
-  def fill(self, frames: dict) -> dict:
-    """reset() of the env: every env's history is the frame."""
+  def fill(self, frames: dict, rand=None, randn=None) -> dict:
+    """reset() of the env: the reference's reset(all) then compute, so every env's bias is redrawn, the noise drawn
+    (from fresh W, N of rand and randn) and every env's history is the frame.  The first call also does what the
+    reference's first reset(all) and first compute do to a bias: one draw per env into the (n, 1) bias, then a
+    per-element draw on top of it for a per-component bias (noise_model.py _initialize_bias_shape)."""
     f = frames["policy"]
-    return self.update(frames, torch.ones(f.shape[0], dtype=torch.bool, device=f.device))
+    all_ = torch.ones(f.shape[0], dtype=torch.bool, device=f.device)
+    if not self.noisy:
+      return self.update(frames, all_)
+    self.draw(rand, randn)
+    if self._shaped:
+      return self.update(frames, all_)
+    for g in self.noisy:
+      if self.groups[g].bias is not None:
+        self.groups[g].redraw_bias(None, self.W, self.N, first=True)
+    self.draw(rand, randn)
+    for g in self.noisy:
+      if self.groups[g].bias is not None:
+        self.groups[g].redraw_bias(None, self.W, self.N, shape=True)
+    self._shaped = True
+    return self.update(frames, all_, redraw=False)
 
   def bind(self, frames: dict, terminated: torch.Tensor, truncated: torch.Tensor) -> None:
     """Build the argument block of b2_obs_history over the fused path's frame buffers (persistent tensors)."""
@@ -236,6 +385,13 @@ class Observations:
     A.ngroup = len(self.active)
     for k, g in enumerate(self.active):
       self.groups[g].native_group(A.group[k], frames[g])
+      if self.groups[g].noisy:
+        self.groups[g].native_noise(A.noise[k], frames["critic"])
+    for name, t in (("W", self.W), ("N", self.N), ("param", self.param_row)):
+      if t is not None:
+        setattr(A, name, t.data_ptr())
+    A.nW, A.nN = self.nW, self.nN
+    A.nparam = 0 if self.param_row is None else self.param_row.numel()
     self._args, self._keep = A, (frames, terminated, truncated)
 
   def run_native(self, sim, frames: dict) -> dict:

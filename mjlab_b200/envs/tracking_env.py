@@ -36,6 +36,7 @@ from mjlab_b200.asset_zoo import g1, load_compiled
 from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply, quat_apply_inverse, quat_mul
 from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
 from mjlab_b200.envs.motion import MotionClip
+from mjlab_b200.envs.noise import TaskNoise, tracking_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.envs.velocity_env import _resolve
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg, native
@@ -174,6 +175,10 @@ class TrackingEnvCfg:
       _check_range6("push_velocity_range", self.push_velocity_range)
     if not self.episode_length_s > 0:
       raise ValueError(f"episode_length_s must be positive, not {self.episode_length_s}")
+    on = self.observations.policy.enable_corruption
+    if on is not None and bool(on) != bool(self.policy_corruption):
+      raise ValueError(f"observations.policy.enable_corruption={on} contradicts policy_corruption="
+                       f"{self.policy_corruption}; set one of them")
 
 
 _NO_RSI = ((0.0, 0.0),) * 6  # an empty pose_range / velocity_range dict of MotionCommandCfg: every offset 0
@@ -315,6 +320,9 @@ class TrackingFlatEnv:
   def _rand(self, *shape):
     return torch.rand(shape, generator=self.gen, device=self.device)
 
+  def _randn(self, *shape):
+    return torch.randn(shape, generator=self.gen, device=self.device)
+
   def _clip(self, name):
     return self.motion[name][self.time_steps]
 
@@ -329,8 +337,11 @@ class TrackingFlatEnv:
     self.reward_stds = [float(getattr(rc, t + "_std")) for t in TRACKING_TERMS]
     self.term_thresholds = [getattr(tc, t) for t in TERMINATION_TERMS[1:]]
     self._push_r = None if cfg.push_velocity_range is None else torch.tensor(cfg.push_velocity_range, **f32)
-    self.obs_groups = Observations(cfg.observations, obs_terms(self.nu, len(BODY_NAMES), cfg.policy_state_estimation),
-                                   n, self.device)
+    terms = obs_terms(self.nu, len(BODY_NAMES), cfg.policy_state_estimation)
+    # noise-configured groups: the task's default noise (policy as policy_corruption, critic none) on the critic frame
+    task_noise = TaskNoise(tracking_defaults(), {"policy": bool(cfg.policy_corruption), "critic": False},
+                           terms["critic"])
+    self.obs_groups = Observations(cfg.observations, terms, n, self.device, task_noise)
     self.nobs, self.nobs_critic = self.obs_groups.width("policy"), self.obs_groups.width("critic")  # elements per env
     self.episode_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
     self.finished_sums = torch.zeros(n, len(REWARD_TERMS), **f32)
@@ -537,7 +548,7 @@ class TrackingFlatEnv:
     self.sim.forward()
     self._update_command()
     policy, critic = self.observations()
-    out = self.obs_groups.fill({"policy": policy, "critic": critic})
+    out = self.obs_groups.fill({"policy": policy, "critic": critic}, self._rand, self._randn)
     return out["policy"], out["critic"]
 
   def enable_cuda_graph(self) -> None:
@@ -566,6 +577,7 @@ class TrackingFlatEnv:
     n = self.num_envs
     U = self._rand(n, 48 + 4 * self.nu)  # B2_TRACKENV_NU: every random number of this env step (include/b2sim.h)
     self.events.draw(self._rand)         # (and those of the reset and interval events, when there are any)
+    self.obs_groups.draw(self._rand, self._randn)  # (and the observation noise's, when a term draws)
     if self.native_mdp:
       return self._step_native(action, U)
     return self._step_torch(action, U)

@@ -21,6 +21,7 @@ import torch
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
 from mjlab_b200.entity_data import EntityIndexing
 from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
+from mjlab_b200.envs.noise import TaskNoise, velocity_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
 
@@ -285,7 +286,10 @@ class VelocityFlatEnv:
     self.push_time_left.copy_(self._rand(n) * (hi_t - lo_t) + lo_t)
     self._init_rewards()
     self._init_command(jnames)
-    self.obs_groups = Observations(cfg.observations, {g: obs_terms(self.nu) for g in ("policy", "critic")}, n, device)
+    # noise-configured groups: the task's default noise (policy corrupted, critic not) on the noise-free critic frame
+    task_noise = TaskNoise(velocity_defaults(), {"policy": True, "critic": False}, obs_terms(self.nu))
+    self.obs_groups = Observations(cfg.observations, {g: obs_terms(self.nu) for g in ("policy", "critic")}, n, device,
+                                   task_noise)
     self.nobs, self.nobs_critic = self.obs_groups.width("policy"), self.obs_groups.width("critic")  # elements per env
     if self.native_mdp:
       self._init_native()
@@ -294,6 +298,9 @@ class VelocityFlatEnv:
   # -- helpers -----------------------------------------------------------------------------------
   def _rand(self, *shape):
     return torch.rand(shape, generator=self.gen, device=self.device)
+
+  def _randn(self, *shape):
+    return torch.randn(shape, generator=self.gen, device=self.device)
 
   def _draw(self) -> torch.Tensor:
     """The step's uniform numbers, one launch (layout: include/b2sim.h B2VelEnvArgs.U): 0-1 reset xy, 2 yaw,
@@ -666,7 +673,7 @@ class VelocityFlatEnv:
     self.sim.forward()
     self._update_command(all_, U, metrics=False)
     frame = self.observations()
-    return self.obs_groups.fill({"policy": frame, "critic": frame})["policy"]
+    return self.obs_groups.fill({"policy": frame, "critic": frame}, self._rand, self._randn)["policy"]
 
   def enable_cuda_graph(self) -> None:
     """Capture one whole env step (ctrl write, 4 sub-steps, MDP glue, masked reset + forward) in a
@@ -706,6 +713,7 @@ class VelocityFlatEnv:
     self._action_in.copy_(action)
     self._U.copy_(self._draw())
     self.events.draw(self._rand)
+    self.obs_groups.draw(self._rand, self._randn)
     native.check(sim._lib.b2_velenv_pre(
       sim._h, ctypes.c_void_p(self._action_in.data_ptr()), ctypes.c_void_p(self.default_joint_pos.data_ptr()),
       ctypes.c_void_p(self.action_scale.data_ptr()), sim._stream()))
@@ -735,6 +743,7 @@ class VelocityFlatEnv:
     """Reference implementation of the same step in torch ops (also the checker of the fused kernels)."""
     U = self._draw()
     self.events.draw(self._rand)
+    self.obs_groups.draw(self._rand, self._randn)
     # JointPositionAction: target = default + scale * action (joint_actions.py:85-103)
     self.sim.data.ctrl[:] = self.default_joint_pos + self.action_scale * action
     self.sim.step_n(self.cfg.decimation)

@@ -117,10 +117,27 @@ class B2ObsHistGroup(ctypes.Structure):
               + [("term", B2ObsHistTerm * OBSHIST_NTERM)])
 
 
+NOISE_NONE, NOISE_CONSTANT, NOISE_UNIFORM, NOISE_GAUSSIAN = 0, 1, 2, 3  # B2_NOISE_* classes (add / scale / abs: 0-2)
+
+
+class B2ObsNoiseTerm(ctypes.Structure):
+  _fields_ = [(n, ctypes.c_int32) for n in ("col", "noise", "noise_op", "noise_p0", "noise_p1", "noise_draw", "bias",
+                                            "bias_op", "bias_p0", "bias_p1", "bias_draw", "bias_shared")]
+
+
+class B2ObsNoiseGroup(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_void_p) for n in ("source", "bias")]
+              + [(n, ctypes.c_int32) for n in ("source_width", "pad_")]
+              + [("term", B2ObsNoiseTerm * OBSHIST_NTERM)])
+
+
 class B2ObsHistArgs(ctypes.Structure):
   _fields_ = ([(n, ctypes.c_void_p) for n in ("terminated", "truncated", "scale")]
               + [(n, ctypes.c_int32) for n in ("nscale", "ngroup")]
-              + [("group", B2ObsHistGroup * OBSHIST_NGROUP)])
+              + [("group", B2ObsHistGroup * OBSHIST_NGROUP)]
+              + [(n, ctypes.c_void_p) for n in ("W", "N", "param")]
+              + [(n, ctypes.c_int32) for n in ("nW", "nN", "nparam")]
+              + [("noise", B2ObsNoiseGroup * OBSHIST_NGROUP)])
 
 
 EVENTS_NTERM = 16  # B2_EVENTS_NTERM: reset and interval terms per b2_events launch
