@@ -115,6 +115,13 @@ int b2_step_host(b2_sim* sim, const float* ctrl_host, int nsteps, float* qpos_ho
 #define B2_VELENV_NU(nu) (16 + 9 + 2 * (nu))
 #define B2_VELENV_NTERM 14 /* reward terms with an episode sum (B2VelEnvArgs.episode_sums) */
 #define B2_VELENV_NSTAGE 8 /* stages of the command-velocity curriculum (B2VelEnvArgs.n_stage) */
+#define B2_VELENV_NRESET 4 /* reset state terms (B2VelEnvArgs.reset_term) */
+enum { B2_RESET_ROOT = 0, B2_RESET_JOINTS = 1 };
+typedef struct B2VelResetTerm {
+  int32_t kind, col, count;       /* B2_RESET_ROOT (count 12) / B2_RESET_JOINTS (count joints, <= 32) */
+  int32_t joint[32];              /* JOINTS: actuated joint indices 0..nu-1 */
+  float lo[12], span[12];         /* ROOT: per draw; JOINTS: [0] position scale, [1] velocity scale */
+} B2VelResetTerm;
 typedef struct B2VelEnvArgs {
   const float* action;            /* [n][nu] */
   const float* U;                 /* [n][B2_VELENV_NU(nu)] uniforms in [0,1): 0-1 reset xy, 2 yaw, 3-5 command, 6 heading
@@ -211,6 +218,20 @@ typedef struct B2VelEnvArgs {
   float* metric_yaw;              /* [n] in/out: error_vel_yaw */
   float* finished_metrics;        /* [n][2] out: (xy, yaw) of the episode a done env just ended */
   float metric_steps;             /* resampling_time_range[1] / step_dt */
+  /* (appended) push_off = 1: no built-in push; push_time_left is neither advanced nor redrawn and push_vel is unread */
+  int32_t push_off;
+  /* (appended) reset state terms (reset_root_state_uniform, reset_joints_by_scale, envs/mdp/events.py:43-124), run in
+   * table order in a reset env after the built-in reset (and the terrain curriculum), before the command and the
+   * observations.  Draws: d_k = lo[k] + ev_V[w][col + k] span[k] (one fp32 product, then one fp32 sum).
+   *   ROOT (12 draws: x y z roll pitch yaw of the pose, then of the velocity): qpos[0:3] = default_qpos[0:3] + d[0:3]
+   *     + env_origins[w]; qpos[3:7] = default_qpos[3:7] * quat(euler xyz d[3:6]); qvel[0:3] = d[6:9];
+   *     qvel[3:6] = R(qpos[3:7])^T d[9:12].
+   *   JOINTS (count joints, joint[j] in 0..nu-1; draws: count position scales, then count velocity scales):
+   *     qpos[7 + a] = clamp(default_joint_pos[a] lo[0]-span[0] draw, soft_lo[a], soft_hi[a]); qvel[6 + a] = 0 times
+   *     the velocity draw (the default joint velocity is 0). */
+  const float* ev_V;              /* [n][ev_v_width] the events' uniforms of this step (B2EventArgs.V) */
+  int32_t ev_v_width, n_reset;    /* n_reset <= B2_VELENV_NRESET; 0 leaves the block unread */
+  B2VelResetTerm reset_term[B2_VELENV_NRESET];
 } B2VelEnvArgs;
 int b2_velenv_pre(b2_sim* sim, const float* action, const float* default_joint_pos,
                   const float* action_scale, void* cuda_stream);
@@ -401,6 +422,7 @@ int b2_obs_history(b2_sim* sim, const B2ObsHistArgs* args, void* cuda_stream);
  * `field`, the field's index in the library's model-field table (b2_field_name(sim, B2_MODEL, field)).  The field must
  * be a float model field with a per-world copy (b2_expand_model_field) and every offset inside its row. */
 #define B2_EVENTS_NTERM 16   /* reset and interval terms per launch */
+#define B2_EVENTS_NSTATE 8   /* state terms per launch (B2EventArgs.state) */
 enum { B2_EVENT_RESET = 0, B2_EVENT_INTERVAL = 1 };
 enum { B2_EVENT_ADD = 0, B2_EVENT_SCALE = 1, B2_EVENT_ABS = 2 };
 enum { B2_EVENT_UNIFORM = 0, B2_EVENT_LOG_UNIFORM = 1 };
@@ -415,6 +437,15 @@ typedef struct B2EventElem {
   int32_t offset;                 /* element index in the world's row of the field (element * width + axis) */
   float lo, span;                 /* the draw lo + u span (LOG_UNIFORM: of the logarithm) */
 } B2EventElem;
+enum { B2_EVENT_PUSH = 0, B2_EVENT_WRENCH = 1 };
+typedef struct B2EventStateTerm {
+  int32_t kind, mode;             /* B2_EVENT_PUSH / B2_EVENT_WRENCH; B2_EVENT_RESET / B2_EVENT_INTERVAL */
+  int32_t col, count;             /* first V column; PUSH: 6, WRENCH: bodies */
+  int32_t first, timer;           /* WRENCH: first entry of bodies; INTERVAL: row of timers */
+  float lo[2], span[2];           /* WRENCH: force (0) and torque (1) draws */
+  float lo6[6], span6[6];         /* PUSH: the draw of each axis */
+  float interval_lo, interval_span; /* INTERVAL: the timer's draw lo + u span */
+} B2EventStateTerm;
 typedef struct B2EventArgs {
   const unsigned char* terminated; /* [n] this env step's terminations */
   const unsigned char* truncated;  /* [n] this env step's time-outs */
@@ -424,6 +455,24 @@ typedef struct B2EventArgs {
   int32_t v_width, ninterval, nelem, nterm;
   float step_dt;
   B2EventTerm term[B2_EVENTS_NTERM];
+  /* State terms (push_by_setting_velocity, apply_external_force_torque, envs/mdp/events.py:127-164), run after the
+   * terms above, in table order.  They fire as the terms above do (mode RESET or INTERVAL; the timer of an INTERVAL
+   * state term is row `timer` of timers, a row no term above uses).
+   *   clear_xfrc: a reset env's xfrc_applied row is zeroed first (Entity.reset -> clear_state).
+   *   WRENCH: `count` bodies, bodies[first .. first + count); force axis a of body j is lo[0] + V[w][col + 3 j + a]
+   *     span[0], torque axis a is lo[1] + V[w][col + 3 count + 3 j + a] span[1]; they are written to
+   *     xfrc_applied[w][bodies[first + j]][a] and [3 + a].  The timer's redraw is column col + 6 count.
+   *   PUSH: count = 6; d_k = lo6[k] + V[w][col + k] span6[k] (x y z roll pitch yaw).  The root's world velocity
+   *     (lin, ang) is taken from cvel, xpos and subtree_com of root_body (compute_velocity_from_cvel) with its
+   *     orientation xquat[root_body], or, in an env whose `refreshed` byte is set (its state was rewritten this step
+   *     and the env's masked forward after this launch recomputes it), from qvel[0:3] and R(q) qvel[3:6] with q the
+   *     normalised qpos[3:7].  Then qvel[0:3] = lin + d[0:3] and qvel[3:6] = R(q)^T (ang + d[3:6]).  The timer's
+   *     redraw is column col + 6.
+   * (appended to B2EventArgs: every offset above is unchanged) */
+  const unsigned char* refreshed; /* [n] PUSH: envs the masked forward after this launch recomputes */
+  const int32_t* bodies;          /* [nbodies] WRENCH: body ids, term by term */
+  int32_t nstate, nbodies, clear_xfrc, root_body;
+  B2EventStateTerm state[B2_EVENTS_NSTATE];
 } B2EventArgs;
 int b2_events(b2_sim* sim, const B2EventArgs* args, void* cuda_stream);
 

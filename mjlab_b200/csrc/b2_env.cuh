@@ -84,6 +84,46 @@ __device__ __forceinline__ void b2e_geom_vel(const DevData& dd, int w, int g, in
   z = p[2];
 }
 
+// The reset state terms of a reset env (B2VelEnvArgs.reset_term), after the built-in reset has written the env's rows
+__device__ __forceinline__ void b2e_reset_terms(const B2VelEnvArgs& A, float* qpos, float* qvel, int w, int lane) {
+  const float* V = A.ev_V + (size_t)w * A.ev_v_width;
+  for (int t = 0; t < A.n_reset; t++) {
+    const int col = A.reset_term[t].col, count = A.reset_term[t].count;
+    if (A.reset_term[t].kind == B2_RESET_ROOT) {
+      if (lane == 0) {
+        float d[12];
+#pragma unroll
+        for (int k = 0; k < 12; k++) d[k] = b2e_add_rn(b2e_mul_rn(V[col + k], A.reset_term[t].span[k]), A.reset_term[t].lo[k]);
+        const float* org = A.env_origins + 3 * (size_t)w;
+#pragma unroll
+        for (int k = 0; k < 3; k++) qpos[k] = b2e_add_rn(b2e_add_rn(A.default_qpos[k], d[k]), org[k]);
+        const float cr = cosf(d[3] * 0.5f), sr = sinf(d[3] * 0.5f), cp = cosf(d[4] * 0.5f), sp = sinf(d[4] * 0.5f);
+        const float cy = cosf(d[5] * 0.5f), sy = sinf(d[5] * 0.5f);
+        const float e[4] = {cy * cr * cp + sy * sr * sp, cy * sr * cp - sy * cr * sp, cy * cr * sp + sy * sr * cp,
+                            sy * cr * cp - cy * sr * sp};
+        const float* a = A.default_qpos + 3;
+        float q[4] = {a[0] * e[0] - a[1] * e[1] - a[2] * e[2] - a[3] * e[3], a[0] * e[1] + a[1] * e[0] + a[2] * e[3] - a[3] * e[2],
+                      a[0] * e[2] - a[1] * e[3] + a[2] * e[0] + a[3] * e[1], a[0] * e[3] + a[1] * e[2] - a[2] * e[1] + a[3] * e[0]};
+        const float ang[3] = {d[9], d[10], d[11]};
+        float ab[3];
+        b2e_rot_inv(q, ang, ab);
+        qpos[3] = q[0]; qpos[4] = q[1]; qpos[5] = q[2]; qpos[6] = q[3];
+        qvel[0] = d[6]; qvel[1] = d[7]; qvel[2] = d[8]; qvel[3] = ab[0]; qvel[4] = ab[1]; qvel[5] = ab[2];
+      }
+    } else {
+      const float plo = A.reset_term[t].lo[0], pspan = A.reset_term[t].span[0];
+      const float vlo = A.reset_term[t].lo[1], vspan = A.reset_term[t].span[1];
+      for (int j = lane; j < count; j += 32) {
+        const int a = A.reset_term[t].joint[j];
+        const float jp = b2e_mul_rn(A.default_joint_pos[a], b2e_add_rn(b2e_mul_rn(V[col + j], pspan), plo));
+        qpos[7 + a] = fminf(fmaxf(jp, A.soft_lo[a]), A.soft_hi[a]);
+        qvel[6 + a] = b2e_mul_rn(0.f, b2e_add_rn(b2e_mul_rn(V[col + count + j], vspan), vlo));
+      }
+    }
+    __syncwarp();
+  }
+}
+
 // feet_air_time (tasks/velocity/mdp/rewards.py:52-146) on one lane per foot: advances the foot's state (zeroed when
 // the env is done, as reset(env_ids) does) and returns the warp's reward before the command scale.
 __device__ __forceinline__ float b2e_air_time(const B2VelEnvArgs& A, const float* sd, int w, int lane, bool done) {
@@ -127,7 +167,7 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   const float down[3] = {0.f, 0.f, -1.f};
   float q[4] = {qpos[3], qpos[4], qpos[5], qpos[6]}, gb[3], lb[3];
   float c0 = cmd[0], c1 = cmd[1], c2 = cmd[2];
-  float ctl = A.cmd_time_left[w] - A.step_dt, tl = A.push_time_left[w] - A.step_dt;
+  float ctl = A.cmd_time_left[w] - A.step_dt, tl = A.push_time_left[w] - (A.push_off ? 0.f : A.step_dt);
   float htarget = A.heading_target[w];
   bool standing = A.is_standing[w] != 0;
   const float v0 = qvel[0], v1 = qvel[1], v2 = qvel[2], wz = qvel[5];
@@ -249,6 +289,10 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
     }
     for (int a = lane; a < nu; a += 32) { ctrl[a] = A.default_joint_pos[a]; last[a] = 0.f; }
     for (int i = lane; i < nv; i += 32) qvel[i] = 0.f;
+    if (A.n_reset > 0) {
+      __syncwarp();  // the built-in rows are written; the terms replace theirs
+      b2e_reset_terms(A, qpos, qvel, w, lane);
+    }
     ep = 0;
   } else {
     for (int a = lane; a < nu; a += 32) last[a] = act[a];
@@ -292,7 +336,7 @@ __global__ void b2_velenv_post_kernel(DevData dd, int nq, int nv, int nu, B2VelE
   }
   // interval event: push_by_setting_velocity
   float pv0 = qvel[0], pv1 = qvel[1];
-  const bool push = tl <= 0.f;
+  const bool push = !A.push_off && tl <= 0.f;
   if (push) {
     pv0 = (U[9] * 2.f - 1.f) * A.push_vel;
     pv1 = (U[10] * 2.f - 1.f) * A.push_vel;

@@ -1116,6 +1116,20 @@ int b2_velenv_post(b2_sim* s, const B2VelEnvArgs* args, void* stream) {
       !a.finished_metrics || !(a.metric_steps > 0.f))
     return fail("b2_velenv_post: needs episode_sums, finished_sums, posture_inv_std2, metric_xy, metric_yaw, "
                 "finished_metrics and metric_steps > 0");
+  if (a.n_reset < 0 || a.n_reset > B2_VELENV_NRESET || (a.n_reset > 0 && (!a.ev_V || a.ev_v_width < 1)))
+    return fail("b2_velenv_post: the reset state terms need 0 <= n_reset <= B2_VELENV_NRESET and the events' V");
+  for (int t = 0; t < a.n_reset; t++) {
+    const B2VelResetTerm& T = a.reset_term[t];
+    const std::string which = "b2_velenv_post: reset term " + std::to_string(t);
+    if (T.kind != B2_RESET_ROOT && T.kind != B2_RESET_JOINTS) return fail(which + " has an unknown kind code");
+    const int draws = T.kind == B2_RESET_ROOT ? 12 : 2 * T.count;
+    if ((T.kind == B2_RESET_ROOT ? T.count != 12 : (T.count < 1 || T.count > 32)) || T.col < 0 ||
+        (long long)T.col + draws > a.ev_v_width)
+      return fail(which + " reads V columns outside the row or has a bad count");
+    for (int j = 0; T.kind == B2_RESET_JOINTS && j < T.count; j++)
+      if (T.joint[j] < 0 || T.joint[j] >= s->hm.nu)
+        return fail(which + " names joint " + std::to_string(T.joint[j]) + ", outside 0..nu-1");
+  }
   DeviceGuard guard(s->device);
   b2_velenv_post_kernel<<<(s->nworld + 3) / 4, 128, 0, (cudaStream_t)stream>>>(  // one warp per environment
       s->hd, s->hm.nq, s->hm.nv, s->hm.nu, a);
@@ -1282,10 +1296,11 @@ int b2_obs_history(b2_sim* s, const B2ObsHistArgs* args, void* stream) {
 
 static int events_check(b2_sim* s, const B2EventArgs* a, B2EventFields* F) {
   if (!s || !a) return fail("b2_events: bad arguments");
-  if (!a->terminated || !a->truncated || !a->V || !a->elem || a->v_width < 1 || a->nterm < 1 ||
-      a->nterm > B2_EVENTS_NTERM || a->ninterval < 0 || a->nelem < 1 || !(a->step_dt > 0.0f))
+  if (!a->terminated || !a->truncated || !a->V || (a->nterm > 0 && !a->elem) || a->v_width < 1 || a->nterm < 0 ||
+      a->nterm > B2_EVENTS_NTERM || a->nstate < 0 || a->nstate > B2_EVENTS_NSTATE || a->nterm + a->nstate < 1 ||
+      a->ninterval < 0 || a->nelem < 0 || !(a->step_dt > 0.0f))
     return fail("b2_events: needs terminated, truncated, V (v_width >= 1), the entry table, "
-                "1 <= nterm <= B2_EVENTS_NTERM and step_dt > 0");
+                "0 <= nterm <= B2_EVENTS_NTERM, 0 <= nstate <= B2_EVENTS_NSTATE, a term and step_dt > 0");
   long long first = 0;
   int ninterval = 0;
   for (int t = 0; t < a->nterm; t++) {
@@ -1312,16 +1327,61 @@ static int events_check(b2_sim* s, const B2EventArgs* a, B2EventFields* F) {
     ninterval += interval;
   }
   if (first != a->nelem) return fail("b2_events: the terms' counts do not add up to nelem");
+  long long nbodies = 0;
+  int last_timer = ninterval - 1;  // the state terms' rows follow the field terms', in table order
+  for (int t = 0; t < a->nstate; t++) {
+    const B2EventStateTerm& S = a->state[t];
+    const std::string which = "b2_events: state term " + std::to_string(t);
+    if ((S.kind != B2_EVENT_PUSH && S.kind != B2_EVENT_WRENCH) ||
+        (S.mode != B2_EVENT_RESET && S.mode != B2_EVENT_INTERVAL) || (S.kind == B2_EVENT_PUSH && S.mode != B2_EVENT_INTERVAL))
+      return fail(which + " has an unknown kind or mode code (a push is an interval term)");
+    const bool interval = S.mode == B2_EVENT_INTERVAL;
+    const long long draws = S.kind == B2_EVENT_PUSH ? 6 : 6LL * S.count;
+    if ((S.kind == B2_EVENT_PUSH ? S.count != 6 : S.count < 1) || S.col < 0 ||
+        (long long)S.col + draws + (interval ? 1 : 0) > a->v_width)
+      return fail(which + " reads V columns outside the block or has a bad count");
+    if (S.kind == B2_EVENT_WRENCH) {
+      if (S.first != nbodies) return fail(which + "'s bodies do not follow the previous term's in the body table");
+      nbodies += S.count;
+    }
+    if (interval) {
+      if (S.timer <= last_timer || S.timer >= a->ninterval || !a->timers)
+        return fail(which + " needs a timer row of its own, after the previous interval term's and below ninterval");
+      last_timer = S.timer;
+      if (!(S.interval_lo >= 0.0f && S.interval_span >= 0.0f && S.interval_lo + S.interval_span < INFINITY))
+        return fail(which + " needs a finite interval with 0 <= lo and span >= 0");
+      ninterval++;
+    }
+    if (S.kind == B2_EVENT_PUSH && (!a->refreshed || a->root_body < 1 || a->root_body >= s->hm.nbody))
+      return fail(which + ": a push needs the refreshed mask and a root_body of the model");
+  }
+  if (nbodies != a->nbodies || (nbodies > 0 && !a->bodies))
+    return fail("b2_events: the wrench terms' counts do not add up to nbodies");
+  if ((a->clear_xfrc || nbodies > 0) && (!s->hd.xfrc_applied.p || s->hd.xfrc_applied.stride < 6 * s->hm.nbody))
+    return fail("b2_events: the wrench terms need a per-world xfrc_applied");
   if (ninterval > a->ninterval || (ninterval > 0 && !a->timers))
     return fail("b2_events: the interval terms need their timers ([ninterval][n])");
+  const DevData& d = s->hd;
+  F->qpos = d.qpos.p; F->qvel = d.qvel.p; F->xfrc = d.xfrc_applied.p; F->xpos = d.xpos.p; F->xquat = d.xquat.p;
+  F->subtree_com = d.subtree_com.p; F->cvel = d.cvel.p;
+  F->qpos_s = d.qpos.stride; F->qvel_s = d.qvel.stride; F->xfrc_s = d.xfrc_applied.stride; F->xpos_s = d.xpos.stride;
+  F->xquat_s = d.xquat.stride; F->subtree_com_s = d.subtree_com.stride; F->cvel_s = d.cvel.stride;
   // The entry table is device memory: it is read back and checked the first time this sim sees it with these fields
   // and counts (a synchronising copy, so outside a stream capture), and taken as unchanged after that, so that the
   // calls an env step captures read nothing back.
-  std::vector<long long> key = {(long long)(uintptr_t)a->elem, a->nelem};
+  std::vector<long long> key = {(long long)(uintptr_t)a->elem, a->nelem, (long long)(uintptr_t)a->bodies, a->nbodies};
   for (int t = 0; t < a->nterm; t++) key.insert(key.end(), {a->term[t].field, a->term[t].count});
   if (key == s->events_checked) return 0;
   std::vector<B2EventElem> elem(a->nelem);
-  CUDA_OK(cudaMemcpy(elem.data(), a->elem, sizeof(B2EventElem) * elem.size(), cudaMemcpyDeviceToHost));
+  if (a->nelem)
+    CUDA_OK(cudaMemcpy(elem.data(), a->elem, sizeof(B2EventElem) * elem.size(), cudaMemcpyDeviceToHost));
+  std::vector<int32_t> bodies(a->nbodies);
+  if (a->nbodies)
+    CUDA_OK(cudaMemcpy(bodies.data(), a->bodies, sizeof(int32_t) * bodies.size(), cudaMemcpyDeviceToHost));
+  for (int32_t b : bodies)
+    if (b < 1 || b >= s->hm.nbody)
+      return fail("b2_events: a wrench term names body " + std::to_string(b) + ", outside the model's bodies 1.." +
+                  std::to_string(s->hm.nbody - 1));
   first = 0;
   for (int t = 0; t < a->nterm; t++) {
     const Field& f = s->model_fields[a->term[t].field];

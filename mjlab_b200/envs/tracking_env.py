@@ -34,7 +34,8 @@ import torch.nn.functional as F
 
 from mjlab_b200.asset_zoo import g1, load_compiled
 from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply, quat_apply_inverse, quat_mul
-from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
+from mjlab_b200.envs.events import (RESET_STATE_TERMS, ApplyExternalForceTorqueCfg, Events, EventsCfg,
+                                    PushBySettingVelocityCfg, RandomizeFieldCfg)
 from mjlab_b200.envs.motion import MotionClip
 from mjlab_b200.envs.noise import TaskNoise, tracking_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
@@ -169,6 +170,14 @@ class TrackingEnvCfg:
     self.rewards.check()
     self.terminations.check()
     self.events.check()
+    for t in self.events.terms:
+      if isinstance(t, PushBySettingVelocityCfg) and self.push_velocity_range is not None:
+        raise ValueError("a PushBySettingVelocityCfg term needs push_velocity_range=None: the built-in push also "
+                         "writes the root velocity, and it cannot take the term's place in the list order")
+      if isinstance(t, RESET_STATE_TERMS) or (isinstance(t, ApplyExternalForceTorqueCfg) and t.mode == "reset"):
+        raise ValueError(f"a {type(t).__name__} term of mode 'reset' is a no-op in the tracking env: the motion "
+                         "command's RSI rewrites the root, the joints and clears the wrenches (clear_state) after the "
+                         "reset events")
     _check_range6("pose_range", self.pose_range)
     _check_range6("velocity_range", self.velocity_range)
     if self.push_velocity_range is not None:
@@ -278,7 +287,8 @@ class TrackingFlatEnv:
       [(idx // cols - (cols - 1) / 2) * cfg.env_spacing, (idx % cols - (cols - 1) / 2) * cfg.env_spacing,
        torch.zeros(n, device=dev)], dim=1).float()
     # ---- domain randomisation: the task's startup terms, then cfg.events; the fields they name get a per-world copy
-    self.events = Events(startup_events(cfg) + tuple(cfg.events.terms), ix, self.sim, n, self.step_dt, device)
+    self.events = Events(startup_events(cfg) + tuple(cfg.events.terms), ix, self.sim, n, self.step_dt, device,
+                         clear_xfrc=False)  # (the RSI of _resample clears the wrenches)
     self.sim.expand_model_fields(self.events.fields())
     self.events.run_startup(self._rand)
     self.events.draw_timers(self._rand)
@@ -652,7 +662,8 @@ class TrackingFlatEnv:
     self._native_args = A
     self._keep = ptr
     self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
-    self.events.bind(self._term, self._trunc)
+    # (the interval push and wrench run after post2's observations, from the forward's cvel)
+    self.events.bind(self._term, self._trunc, self._done_buf, interval_after_obs=True)
 
   def _step_native(self, action: torch.Tensor, U: torch.Tensor):
     """Two fused kernels around the masked forward (csrc/b2_trackenv.cuh) instead of ~150 torch launches."""
@@ -689,6 +700,7 @@ class TrackingFlatEnv:
     self.events.run_native(sim)
     sim.forward(env_mask=self._done_buf)
     native.check(sim._lib.b2_trackenv_post2(sim._h, ctypes.byref(self._native_args), st))
+    self.events.run_native_after_obs(sim)
     out = self.obs_groups.run_native(sim, {"policy": self._obs, "critic": self._critic})
     return out["policy"], self._reward, self._term, self._trunc, self._extras(out["critic"])
 
@@ -790,6 +802,7 @@ class TrackingFlatEnv:
       self.push_time_left.copy_(torch.where(push, P[:, 6] * (hi_t - lo_t) + lo_t, self.push_time_left))
     policy, critic = self.observations(U[:, 2 * S + 7:])
     out = self.obs_groups.update({"policy": policy, "critic": critic}, terminated | truncated)
+    self.events.step_interval_state()  # the interval push and wrench terms, after the observations
     return out["policy"], reward, terminated, truncated, self._extras(out["critic"])
 
   def close(self):

@@ -20,7 +20,8 @@ import torch
 
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
 from mjlab_b200.entity_data import EntityIndexing
-from mjlab_b200.envs.events import Events, EventsCfg, RandomizeFieldCfg
+from mjlab_b200.envs import events as evm
+from mjlab_b200.envs.events import Events, EventsCfg, PushBySettingVelocityCfg, RandomizeFieldCfg
 from mjlab_b200.envs.noise import TaskNoise, velocity_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
@@ -109,7 +110,7 @@ class VelocityEnvCfg:
   episode_length_s: float = 20.0           # :272
   fall_angle: float = math.radians(70.0)   # :241-243
   push_interval_s: tuple = (1.0, 3.0)      # :156-161
-  push_vel: float = 0.5                    # flat_env_cfg.py:20-24
+  push_vel: float | None = 0.5             # flat_env_cfg.py:20-24; None: no built-in push
   friction_range: tuple = (0.3, 1.2)       # :162-172
   env_spacing: float = 2.5
   terrain: str = "flat"                    # "flat" (plane) | "rough" (box terrain, velocity_env_cfg.py:274-278)
@@ -136,8 +137,19 @@ class VelocityEnvCfg:
   posture_std: dict | None = None
   # clip, scale and history of the policy and critic groups (terms: OBS_TERMS); the defaults leave both as computed
   observations: ObservationsCfg = field(default_factory=ObservationsCfg)
-  # randomize_field events (envs/events.py), run after the startup foot friction of friction_range
+  # event terms (envs/events.py), run after the startup foot friction of friction_range: randomize_field, and the
+  # state terms push_by_setting_velocity (needs push_vel=None) and apply_external_force_torque
   events: EventsCfg = field(default_factory=EventsCfg)
+
+  def __post_init__(self):
+    self.check()
+
+  def check(self) -> None:
+    self.events.check()
+    if self.push_vel is not None and self.events.has(PushBySettingVelocityCfg):
+      raise ValueError("a PushBySettingVelocityCfg term needs push_vel=None: the built-in push also writes the root "
+                       "velocity, and it runs before the observations, where it cannot take the term's place in the "
+                       "list order")
 
 
 def _float32(x) -> float:
@@ -262,10 +274,11 @@ class VelocityFlatEnv:
       self.terrain_level_mean = self.terrain_levels.float().mean()
     # domain randomisation: the task's startup foot friction (velocity_env_cfg.py:162-172), then cfg.events; the
     # fields they name get a per-world copy first
-    cfg.events.check()
+    cfg.check()
     feet = RandomizeFieldCfg("geom_friction", tuple(cfg.friction_range), operation="abs", names=tuple(zoo.FOOT_GEOMS))
     self.events = Events((feet,) + tuple(cfg.events.terms), EntityIndexing.from_model(m, "robot", device), self.sim,
                          n, self.step_dt, device)
+    self.events.set_reset_state(self.default_qpos, self.env_origins, self.soft_lo, self.soft_hi)
     self.sim.expand_model_fields(self.events.fields())
     self.events.run_startup(self._rand)
     self.events.draw_timers(self._rand)
@@ -460,7 +473,8 @@ class VelocityFlatEnv:
     ):
       assert t.is_contiguous()
       setattr(a, name, t.data_ptr())
-    a.step_dt, a.fall_angle, a.push_vel = self.step_dt, self.cfg.fall_angle, self.cfg.push_vel
+    a.step_dt, a.fall_angle = self.step_dt, self.cfg.fall_angle
+    a.push_vel, a.push_off = (0.0, 1) if self.cfg.push_vel is None else (self.cfg.push_vel, 0)
     a.push_lo, a.push_hi = self.cfg.push_interval_s
     a.max_episode_length = self.max_episode_length
     if self.terrain_curriculum:
@@ -503,9 +517,20 @@ class VelocityFlatEnv:
       assert t.is_contiguous()
       setattr(a, name, t.data_ptr())
     a.metric_steps = self.metric_steps
+    resets = self.events.reset_state_terms()  # reset_root_state_uniform / reset_joints_by_scale, in the reset branch
+    if len(resets) > native.VELENV_NRESET:
+      raise ValueError(f"at most {native.VELENV_NRESET} reset root and joint terms, got {len(resets)}")
+    if resets:
+      a.ev_V, a.ev_v_width, a.n_reset = self.events.V.data_ptr(), self.events.v_width, len(resets)
+    for k, t in enumerate(resets):
+      T = a.reset_term[k]
+      T.kind = native.RESET_ROOT if t.kind == evm.ROOT else native.RESET_JOINTS
+      T.col, T.count = t.col, t.count
+      T.joint[:t.count if t.kind == evm.JOINTS else 0] = t.bodies
+      T.lo[:len(t.lo)], T.span[:len(t.span)] = t.lo, t.span
     self._native_args = a
     self.obs_groups.bind({"policy": self._obs, "critic": self._critic}, self._term, self._trunc)
-    self.events.bind(self._term, self._trunc)
+    self.events.bind(self._term, self._trunc, self._done_buf)
 
   def _reset_where(self, mask: torch.Tensor, U: torch.Tensor) -> None:
     """reset_root_state_uniform + reset_joints_by_scale (envs/mdp/events.py:43-124) for masked envs."""
@@ -790,14 +815,16 @@ class VelocityFlatEnv:
     self.sim.forward(env_mask=self._done_buf)  # only the reset envs need new derived quantities here
     self._update_command(done, U)
     self.log_row.copy_(torch.stack([reward, terminated.float(), truncated.float()], dim=1))
-    # interval event: push_by_setting_velocity (events.py:127-143)
-    self.push_time_left -= self.step_dt
-    push = self.push_time_left <= 0
-    pv = (U[:, 9:11] * 2 - 1) * cfg.push_vel
-    d.qvel[:, 0:2] = torch.where(push.unsqueeze(1), pv, d.qvel[:, 0:2])
-    lo_t, hi_t = cfg.push_interval_s
-    self.push_time_left.copy_(torch.where(push, U[:, 11] * (hi_t - lo_t) + lo_t, self.push_time_left))
+    # interval event: push_by_setting_velocity (events.py:127-143), unless push_vel is None
+    if cfg.push_vel is not None:
+      self.push_time_left -= self.step_dt
+      push = self.push_time_left <= 0
+      pv = (U[:, 9:11] * 2 - 1) * cfg.push_vel
+      d.qvel[:, 0:2] = torch.where(push.unsqueeze(1), pv, d.qvel[:, 0:2])
+      lo_t, hi_t = cfg.push_interval_s
+      self.push_time_left.copy_(torch.where(push, U[:, 11] * (hi_t - lo_t) + lo_t, self.push_time_left))
     out = self.obs_groups.update({"policy": self.observations(U), "critic": self.critic_obs}, terminated | truncated)
+    self.events.step_interval_state()  # the interval push and wrench terms, after the observations
     return out["policy"], reward, terminated, truncated, {"critic": out["critic"]}
 
   def close(self):

@@ -48,6 +48,15 @@ VELENV_NTERM = 14  # B2_VELENV_NTERM: reward terms with an episode sum
 VELENV_NSTAGE = 8  # B2_VELENV_NSTAGE: stages of the command-velocity curriculum
 
 
+VELENV_NRESET = 4  # B2_VELENV_NRESET: reset state terms
+RESET_ROOT, RESET_JOINTS = 0, 1  # B2VelResetTerm.kind
+
+
+class B2VelResetTerm(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_int32) for n in ("kind", "col", "count")] + [("joint", ctypes.c_int32 * 32)]
+              + [("lo", ctypes.c_float * 12), ("span", ctypes.c_float * 12)])
+
+
 class B2VelEnvArgs(ctypes.Structure):
   _fields_ = (
     [(n, ctypes.c_void_p) for n in (
@@ -76,6 +85,9 @@ class B2VelEnvArgs(ctypes.Structure):
     + [(n, ctypes.c_void_p) for n in ("step_counter", "posture_inv_std2", "metric_xy", "metric_yaw",
                                       "finished_metrics")]
     + [("metric_steps", ctypes.c_float)]
+    + [("push_off", ctypes.c_int32)]
+    + [("ev_V", ctypes.c_void_p), ("ev_v_width", ctypes.c_int32), ("n_reset", ctypes.c_int32),
+       ("reset_term", B2VelResetTerm * VELENV_NRESET)]
   )
 
 
@@ -154,10 +166,23 @@ class B2EventElem(ctypes.Structure):
   _fields_ = [("offset", ctypes.c_int32), ("lo", ctypes.c_float), ("span", ctypes.c_float)]
 
 
+EVENTS_NSTATE = 8  # B2_EVENTS_NSTATE: state terms per b2_events launch
+EVENT_PUSH, EVENT_WRENCH = 0, 1  # B2EventStateTerm.kind
+
+
+class B2EventStateTerm(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_int32) for n in ("kind", "mode", "col", "count", "first", "timer")]
+              + [("lo", ctypes.c_float * 2), ("span", ctypes.c_float * 2), ("lo6", ctypes.c_float * 6),
+                 ("span6", ctypes.c_float * 6), ("interval_lo", ctypes.c_float), ("interval_span", ctypes.c_float)])
+
+
 class B2EventArgs(ctypes.Structure):
   _fields_ = ([(n, ctypes.c_void_p) for n in ("terminated", "truncated", "V", "timers", "elem")]
               + [(n, ctypes.c_int32) for n in ("v_width", "ninterval", "nelem", "nterm")]
-              + [("step_dt", ctypes.c_float), ("term", B2EventTerm * EVENTS_NTERM)])
+              + [("step_dt", ctypes.c_float), ("term", B2EventTerm * EVENTS_NTERM)]
+              + [(n, ctypes.c_void_p) for n in ("refreshed", "bodies")]
+              + [(n, ctypes.c_int32) for n in ("nstate", "nbodies", "clear_xfrc", "root_body")]
+              + [("state", B2EventStateTerm * EVENTS_NSTATE)])
 
 
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
