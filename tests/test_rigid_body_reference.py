@@ -269,13 +269,14 @@ class Rigid:
         clamped=clamped)
     return out
 
-  def step(self, q, v, ctrl, qfrc_applied, xfrc_applied, h, integrator):
+  def step(self, q, v, ctrl, qfrc_applied, xfrc_applied, h, integrator, qfrc_constraint=0.0):
+    """One step; `qfrc_constraint` (a given constraint force) is added to the smooth forces."""
     S = self.forward(q, v, ctrl, qfrc_applied, xfrc_applied)
     A = S["qM"] + h * np.diag(self.damping)
     if integrator == IMPLICITFAST and self.nu:
       free = ~S["clamped"]
       np.add.at(A, (self.dadr[self.trn][free],) * 2, -h * (self.gear**2 * self.biasprm[:, 2])[free])
-    v1 = np.asarray(v, np.float64) + h * np.linalg.solve(A, S["qfrc_smooth"])
+    v1 = np.asarray(v, np.float64) + h * np.linalg.solve(A, S["qfrc_smooth"] + qfrc_constraint)
     return self.integrate(q, v1, h), v1
 
 
@@ -572,12 +573,15 @@ def ref_forward(refs, st):
 class Backend:
   """The fp64 oracle or an engine (Eng: host emulation or H100) behind one interface."""
 
-  def __init__(self, name, m, n, precision="f64"):
+  def __init__(self, name, m, n, precision="f64", nconmax=None):
+    """`nconmax`: the engine's contact pool over all worlds (the oracle holds the per-world share, and room for
+    four rows per contact)."""
     self.name, self.n = name, n
     if name == "oracle":
-      self.o, self.e = Oracle(m, nworld=n, precision=precision), None
+      maxcon = -(-nconmax // n) if nconmax else 64
+      self.o, self.e = Oracle(m, nworld=n, precision=precision, maxcon=maxcon, njmax=max(300, 4 * maxcon + 128)), None
     else:
-      self.o, self.e = None, Eng(name, m, n)
+      self.o, self.e = None, Eng(name, m, n, nconmax)
 
   def rows(self, rows):
     for k, v in rows.items():
