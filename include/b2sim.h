@@ -14,7 +14,8 @@
  * No torch types cross this boundary: plain pointers, sizes and a CUDA stream handle.
  * All functions return 0 on success, non-zero on error (message via b2_last_error()).
  * Nothing in b2_step/b2_forward allocates, synchronises or touches the host: they only enqueue
- * kernels on the given stream and are CUDA-graph capturable.
+ * kernels on the given stream and are CUDA-graph capturable (an armed NaN guard's kernels write one word of mapped
+ * host memory when they find a non-finite state; b2_nan_guard below).
  */
 #ifndef B2SIM_H_
 #define B2SIM_H_
@@ -475,6 +476,28 @@ typedef struct B2EventArgs {
   B2EventStateTerm state[B2_EVENTS_NSTATE];
 } B2EventArgs;
 int b2_events(b2_sim* sim, const B2EventArgs* args, void* cuda_stream);
+
+/* ---- NaN guard (the reference's NanGuard, utils/nan_guard.py, on the device) -------------------------------------
+ * Armed (flags = B2_NAN_GUARD_ON), every sub-step of b2_step / b2_step_n also
+ *   records, before the sub-step, the qpos / qvel of worlds 0..ncapture-1 as its entry of a ring that keeps the last
+ *   buffer_size entries (sub-steps are numbered from 0 at arming), and
+ *   checks, after it, qpos, qvel, qacc and qacc_warmstart of every world (their nq / nv columns) for NaN / Inf.
+ * The first sub-step that finds one is the detection sub-step: its non-finite worlds are flagged, the host-visible word
+ * (b2_nan_guard_word) becomes 1, and the ring and flags are frozen, so the guard fires once.  This is stream work of the
+ * calls (one launch before the call's first sub-step and one per sub-step and partition after it): a CUDA graph
+ * captured while armed carries it.  While armed, b2_step_n's two partitions join every 8 sub-steps.
+ * Arming (re)starts the guard on fresh buffers: graphs captured before must be re-captured to see them.  flags = 0
+ * disarms: no launch and no allocation from then on (the default; outputs are those of a sim never armed).  Arming
+ * refuses ncapture outside [1, nworld] and buffer_size < 1; it synchronises the device (not capturable). */
+#define B2_NAN_GUARD_ON 1
+int b2_nan_guard(b2_sim* sim, int ncapture, int buffer_size, int flags);
+/* Host address of the guard's word (0, or 1 once a non-finite state was found), readable without synchronising;
+ * NULL when disarmed. */
+const volatile int32_t* b2_nan_guard_word(b2_sim* sim);
+/* Synchronises `cuda_stream` and reads the guard: *detected = the detection sub-step d, or -1.  When d >= 0 and the
+ * buffers are non-NULL: states[k - first][w][0:nq] = qpos and [nq:nq+nv] = qvel of world w before sub-step k, for
+ * k = first .. d (first = max(0, d - buffer_size + 1), w < ncapture); flags[w] = 1 for the worlds non-finite after d. */
+int b2_nan_guard_read(b2_sim* sim, void* cuda_stream, int64_t* detected, float* states, unsigned char* flags);
 
 /* Diagnostics (synchronises `cuda_stream`). */
 int b2_stats(b2_sim* sim, void* cuda_stream, B2Stats* out);

@@ -17,6 +17,7 @@
 #include "b2_trackenv.cuh"
 #include "b2_obshist.cuh"
 #include "b2_events.cuh"
+#include "b2_nanguard.cuh"
 
 static thread_local std::string g_err;
 static int fail(const std::string& msg) {
@@ -70,6 +71,11 @@ struct b2_sim {
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
   size_t smem_bytes = 0;
   std::vector<long long> events_checked;  // b2_events: the entry table last checked (address, size, fields, counts)
+  // NaN guard (b2_nan_guard): the buffers of the last arming; those of earlier armings stay allocated until
+  // b2_destroy, so that a graph captured while they were armed never writes freed memory
+  int guard_on = 0, guard_buffer = 0;
+  B2Guard guard = {};
+  std::vector<void*> host_allocs;
 };
 
 static int pad4(int n) { return (n + 3) & ~3; }
@@ -365,6 +371,22 @@ static int launch(b2_sim* s, bool step, cudaStream_t st, int base = 0, int count
   else
     if (s->has_convex) b2_step_kernel<2><<<grid, 32 * B2_WARPS_PER_CTA, s->smem_bytes, st>>>(s->hm, s->hd);
     else b2_step_kernel<0><<<grid, 32 * B2_WARPS_PER_CTA, s->smem_bytes, st>>>(s->hm, s->hd);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// The NaN guard's work around the sub-steps of one call (b2_nanguard.cuh); nothing while the guard is disarmed.
+static int guard_start(b2_sim* s, cudaStream_t st, int n) {
+  if (!s->guard_on) return 0;
+  b2_guard_start_kernel<<<1, 128, 0, st>>>(s->guard, s->hd, s->hm.nq, s->hm.nv, n);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+static int guard_check(b2_sim* s, cudaStream_t st, int base, int count, int i, int record) {
+  if (!s->guard_on) return 0;
+  b2_guard_check_kernel<<<(count + 3) / 4, 128, 0, st>>>(s->guard, s->hd, s->hm.nq, s->hm.nv, base, count, i, record);
   s->launches++;
   CUDA_OK(cudaGetLastError());
   return 0;
@@ -916,6 +938,7 @@ int b2_destroy(b2_sim* s) {
   if (!s) return 0;
   DeviceGuard guard(s->device);
   for (void* p : s->allocs) cudaFree(p);
+  for (void* p : s->host_allocs) b2g_word_free(p);
   for (int h = 0; h < 2; h++) {
     if (s->side[h]) cudaStreamDestroy(s->side[h]);
     if (s->ev_join[h]) cudaEventDestroy(s->ev_join[h]);
@@ -1034,7 +1057,8 @@ int b2_get_option(b2_sim* s, const char* key, double* v) {
 int b2_step(b2_sim* s, void* stream) {
   if (!s) return fail("b2_step: null sim");
   DeviceGuard guard(s->device);
-  return refresh_kinrec(s, (cudaStream_t)stream) || launch(s, true, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return refresh_kinrec(s, st) || guard_start(s, st, 1) || launch(s, true, st) || guard_check(s, st, 0, s->nworld, 0, 0);
 }
 int b2_forward(b2_sim* s, void* stream) {
   if (!s) return fail("b2_forward: null sim");
@@ -1061,20 +1085,104 @@ int b2_step_n(b2_sim* s, int n, void* stream) {
     // partitions onto internal streams (event fork/join, CUDA-graph capturable). Each partition keeps
     // per-sub-step launches (phase-aligned warps, fresh heavy-first order) while its launch tails overlap the
     // other partition's work.  (1, 3 and 4 partitions measured slower on the H100; DESIGN.md §9.)
+    // While the NaN guard is armed the partitions join every B2_GUARD_CHUNK sub-steps, which bounds how far one can
+    // run ahead of the other's detection (b2_nanguard.cuh).
     int per = (((s->nworld + 1) / 2 + B2_WARPS_PER_CTA - 1) / B2_WARPS_PER_CTA) * B2_WARPS_PER_CTA;
-    CUDA_OK(cudaEventRecord(s->ev_fork, st));
-    for (int h = 0; h < 2; h++) {
-      int base = h * per, count = std::min(per, s->nworld - base);
-      CUDA_OK(cudaStreamWaitEvent(s->side[h], s->ev_fork, 0));
-      for (int i = 0; i < n; i++)
-        if (launch(s, true, s->side[h], base, count, i == n - 1)) return 1;
-      CUDA_OK(cudaEventRecord(s->ev_join[h], s->side[h]));
-      CUDA_OK(cudaStreamWaitEvent(st, s->ev_join[h], 0));
+    const int chunk = s->guard_on ? B2_GUARD_CHUNK : n;
+    for (int c0 = 0; c0 < n; c0 += chunk) {
+      const int m = std::min(chunk, n - c0);
+      if (guard_start(s, st, m)) return 1;
+      CUDA_OK(cudaEventRecord(s->ev_fork, st));
+      for (int h = 0; h < 2; h++) {
+        int base = h * per, count = std::min(per, s->nworld - base);
+        CUDA_OK(cudaStreamWaitEvent(s->side[h], s->ev_fork, 0));
+        for (int i = 0; i < m; i++)
+          if (launch(s, true, s->side[h], base, count, c0 + i == n - 1) ||
+              guard_check(s, s->side[h], base, count, i, i < m - 1))
+            return 1;
+        CUDA_OK(cudaEventRecord(s->ev_join[h], s->side[h]));
+        CUDA_OK(cudaStreamWaitEvent(st, s->ev_join[h], 0));
+      }
     }
     return 0;
   }
+  if (guard_start(s, st, n)) return 1;
   for (int i = 0; i < n; i++)
-    if (launch(s, true, st, 0, -1, i == n - 1)) return 1;
+    if (launch(s, true, st, 0, -1, i == n - 1) || guard_check(s, st, 0, s->nworld, i, i < n - 1)) return 1;
+  return 0;
+}
+
+int b2_nan_guard(b2_sim* s, int ncapture, int buffer_size, int flags) {
+  if (!s) return fail("b2_nan_guard: null sim");
+  if (flags != 0 && flags != B2_NAN_GUARD_ON) return fail("b2_nan_guard: flags must be 0 or B2_NAN_GUARD_ON");
+  if (flags == 0) {
+    s->guard_on = 0;
+    return 0;
+  }
+  if (ncapture < 1 || ncapture > s->nworld || buffer_size < 1)
+    return fail("b2_nan_guard: needs 1 <= ncapture <= nworld (" + std::to_string(s->nworld) + ") and buffer_size >= 1");
+  const long long row = s->hm.nq + s->hm.nv, slots = (long long)buffer_size + B2_GUARD_CHUNK - 1;
+  if (slots * ncapture > (1LL << 36) / row) return fail("b2_nan_guard: the ring of buffer_size x ncapture states is too large");
+  DeviceGuard guard(s->device);
+  CUDA_OK(cudaDeviceSynchronize());  // (work in flight keeps the last arming's buffers, which stay allocated)
+  B2Guard g = {};
+  g.slots = (int)slots;
+  g.ncapture = ncapture;
+  void* p = nullptr;
+  const size_t ring_bytes = sizeof(float) * (size_t)(slots * ncapture * row);
+  CUDA_OK(cudaMalloc(&p, ring_bytes));
+  s->allocs.push_back(p);
+  CUDA_OK(cudaMemset(p, 0, ring_bytes));
+  g.ring = (float*)p;
+  const long long ctl[3] = {0, 0, B2_GUARD_NONE};
+  CUDA_OK(cudaMalloc(&p, sizeof(ctl)));
+  s->allocs.push_back(p);
+  CUDA_OK(cudaMemcpy(p, ctl, sizeof(ctl), cudaMemcpyHostToDevice));
+  g.ctl = (long long*)p;
+  const std::vector<long long> none(s->nworld, B2_GUARD_NONE);
+  CUDA_OK(cudaMalloc(&p, sizeof(long long) * none.size()));
+  s->allocs.push_back(p);
+  CUDA_OK(cudaMemcpy(p, none.data(), sizeof(long long) * none.size(), cudaMemcpyHostToDevice));
+  g.first_bad = (long long*)p;
+  void* dp = nullptr;
+  CUDA_OK(b2g_word_alloc(&p, &dp));
+  s->host_allocs.push_back(p);
+  *(volatile int*)p = 0;
+  g.word = (volatile int*)dp;
+  CUDA_OK(cudaDeviceSynchronize());
+  s->guard = g;
+  s->guard_buffer = buffer_size;
+  s->guard_on = 1;
+  return 0;
+}
+
+const volatile int32_t* b2_nan_guard_word(b2_sim* s) {
+  return s && s->guard_on ? (const volatile int32_t*)s->host_allocs.back() : nullptr;
+}
+
+int b2_nan_guard_read(b2_sim* s, void* stream, int64_t* detected, float* states, unsigned char* flags) {
+  if (!s || !detected) return fail("b2_nan_guard_read: bad arguments");
+  if (!s->guard_on) return fail("b2_nan_guard_read: the NaN guard is not armed");
+  DeviceGuard guard(s->device);
+  CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+  const B2Guard& g = s->guard;
+  long long ctl[3];
+  CUDA_OK(cudaMemcpy(ctl, g.ctl, sizeof(ctl), cudaMemcpyDeviceToHost));
+  *detected = ctl[2] == B2_GUARD_NONE ? -1 : ctl[2];
+  if (*detected < 0) return 0;
+  const long long d = ctl[2], first = std::max(0LL, d - s->guard_buffer + 1);
+  const size_t entry = (size_t)g.ncapture * (s->hm.nq + s->hm.nv);
+  if (states) {
+    std::vector<float> ring((size_t)g.slots * entry);
+    CUDA_OK(cudaMemcpy(ring.data(), g.ring, sizeof(float) * ring.size(), cudaMemcpyDeviceToHost));
+    for (long long k = first; k <= d; k++)
+      memcpy(states + (size_t)(k - first) * entry, ring.data() + (size_t)(k % g.slots) * entry, sizeof(float) * entry);
+  }
+  if (flags) {
+    std::vector<long long> fb(s->nworld);
+    CUDA_OK(cudaMemcpy(fb.data(), g.first_bad, sizeof(long long) * fb.size(), cudaMemcpyDeviceToHost));
+    for (int w = 0; w < s->nworld; w++) flags[w] = fb[w] == d;
+  }
   return 0;
 }
 

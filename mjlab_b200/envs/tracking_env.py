@@ -261,6 +261,7 @@ class TrackingFlatEnv:
     self.model = m = model if model is not None else load_compiled("g1_tracking_flat")
     n = self.num_envs = cfg.num_envs
     self.sim = Simulation(n, cfg.sim, m, device)
+    self._nan_guard = getattr(self.sim, "nan_guard", None)  # (None on a Simulation stand-in without the guard)
     dev = torch.device(device)
     f32 = dict(dtype=torch.float32, device=dev)
     self.nq, self.nv, self.nu = int(m.nq), int(m.nv), int(m.nu)
@@ -577,11 +578,19 @@ class TrackingFlatEnv:
     self._graph = g
 
   def step(self, action: torch.Tensor):
+    """One env step (the captured graph's replay after ``enable_cuda_graph``).  With the sim's NaN guard enabled it then
+    polls the guard without synchronising: a NaN the GPU found in this step's sub-steps is dumped by this call or, when
+    the GPU has not got there yet, by a later step (usually one or two later) or by ``close()``.  The dump's content
+    does not depend on which, because the guard's ring and flags freeze on the device at the detection sub-step."""
     if self._graph is not None:
       self._action_buf.copy_(action, non_blocking=True)
       self._graph.replay()
-      return self._graph_out
-    return self._step_impl(action)
+      out = self._graph_out
+    else:
+      out = self._step_impl(action)
+    if self._nan_guard is not None:
+      self._nan_guard.poll()
+    return out
 
   def _step_impl(self, action: torch.Tensor):
     n = self.num_envs

@@ -185,6 +185,9 @@ class B2EventArgs(ctypes.Structure):
               + [("state", B2EventStateTerm * EVENTS_NSTATE)])
 
 
+NAN_GUARD_ON = 1  # B2_NAN_GUARD_ON: b2_nan_guard's flag that arms the guard
+
+
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
 
 
@@ -244,6 +247,9 @@ def bind(L: ctypes.CDLL) -> ctypes.CDLL:
     "b2_trackenv_bins": ([vp, P(B2TrackEnvArgs), vp], ci),
     "b2_obs_history": ([vp, P(B2ObsHistArgs), vp], ci),
     "b2_events": ([vp, P(B2EventArgs), vp], ci),
+    "b2_nan_guard": ([vp, ci, ci, ci], ci),
+    "b2_nan_guard_word": ([vp], vp),
+    "b2_nan_guard_read": ([vp, vp, P(ctypes.c_int64), vp, vp], ci),
     "b2_stats": ([vp, vp, P(B2Stats)], ci),
     "b2_launch_count": ([vp], ctypes.c_int64),
     "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),

@@ -103,7 +103,8 @@ class Simulation:
     self.step_graph = None
     self.forward_graph = None
     self._graph_dirty = False
-    self.nan_guard = NanGuard(cfg.nan_guard, self.num_envs, self._mj_model)
+    # armed before any graph can be captured, so every graph of this sim carries the guard's stream work
+    self.nan_guard = NanGuard(cfg.nan_guard, self._engine, self._mj_model, self._stream)
 
   # -- plumbing ----------------------------------------------------------------------------------
   def _stream(self) -> ctypes.c_void_p:
@@ -194,24 +195,25 @@ class Simulation:
       native.check(self._lib.b2_forward(self._h, self._stream()))
 
   def step(self) -> None:
+    """One sub-step.  With the NaN guard enabled, and outside a stream capture, it synchronises once at the end and
+    writes the guard's dump if this or an earlier sub-step produced NaN/Inf."""
     if self.use_cuda_graph and self._graph_dirty:
       self.create_graph()
-    with self.nan_guard.watch(self.data):
-      if self.use_cuda_graph and self.step_graph is not None:
-        self.step_graph.replay()
-      else:
-        native.check(self._lib.b2_step(self._h, self._stream()))
+    if self.use_cuda_graph and self.step_graph is not None:
+      self.step_graph.replay()
+    else:
+      native.check(self._lib.b2_step(self._h, self._stream()))
+    self._check_nan_guard()
 
   def step_n(self, n: int) -> None:
     """``n`` sub-steps with ``ctrl`` held (the decimation loop of
-    ``envs/manager_based_rl_env.py:109-114``) in one library call."""
-    if self.nan_guard.enabled and not torch.cuda.is_current_stream_capturing():
-      # the guard copies state to the host, so each sub-step is watched like a `step()` call
-      for _ in range(int(n)):
-        with self.nan_guard.watch(self.data):
-          native.check(self._lib.b2_step(self._h, self._stream()))
-      return
+    ``envs/manager_based_rl_env.py:109-114``) in one library call; the NaN guard as in ``step``."""
     native.check(self._lib.b2_step_n(self._h, int(n), self._stream()))
+    self._check_nan_guard()
+
+  def _check_nan_guard(self) -> None:
+    if self.nan_guard.enabled and not torch.cuda.is_current_stream_capturing():
+      self.nan_guard.check_and_dump()
 
   def stats(self) -> native.B2Stats:
     st = native.B2Stats()
@@ -225,6 +227,7 @@ class Simulation:
     h = getattr(self, "_h", None)
     if h:
       torch.cuda.synchronize(self._dev_index)
+      self.nan_guard.check_and_dump()  # what graphed steps since the last poll found
       # engine memory is about to be freed: drop every cached view and make later field access fail loudly
       for st, br in ((self._wp_data, self._data_bridge), (self._wp_model, self._model_bridge)):
         st._tensors.clear()
