@@ -499,6 +499,34 @@ const volatile int32_t* b2_nan_guard_word(b2_sim* sim);
  * k = first .. d (first = max(0, d - buffer_size + 1), w < ncapture); flags[w] = 1 for the worlds non-finite after d. */
 int b2_nan_guard_read(b2_sim* sim, void* cuda_stream, int64_t* detected, float* states, unsigned char* flags);
 
+/* ---- offscreen frames (the reference's OffscreenRenderer, viewer/offscreen_renderer.py, by ray casting) ------------
+ * One frame of the scene as the last step or forward left it, enqueued on `cuda_stream`; it reads Data and Model and
+ * writes only the output buffers.  Drawn: every geom welded to the world once (world 0's values), and the other geoms
+ * of worlds 0 .. min(noverlay, nworld) - 1 and of env_idx; not drawn: mesh geoms and geoms with alpha 0.  Camera (a
+ * MuJoCo free or tracking camera): forward f = (cos el cos az, cos el sin az, sin el), eye = target - distance f, z up,
+ * vertical field of view 45 degrees, one ray through each pixel centre.  Outputs are row-major from the top row:
+ *   rgb   [height][width][3] uint8, required;
+ *   depth [height][width] float, distance along f, +inf for the background (null: not written);
+ *   seg   [height][width][2] int32 (world, geom), (-1, -1) for the background; welded geoms report world 0 (null: not
+ *         written).
+ * Shading and its constants: DESIGN.md §4.  The first call on a sim builds the list of drawable geoms (it synchronises
+ * the device: not capturable); later calls only launch.  Refused: a size outside 1..4096, env_idx outside
+ * [0, nworld), noverlay < 0, track_body outside [-1, nbody), a null rgb. */
+typedef struct B2RenderArgs {
+  int32_t width, height;          /* pixels, 1..4096 */
+  float lookat[3];                /* camera target when track_body is -1 */
+  int32_t track_body;             /* >= 0: the target is subtree_com of this body in world env_idx (read on the device) */
+  float distance, azimuth, elevation; /* metres, degrees, degrees */
+  int32_t env_idx;                /* the main world */
+  int32_t noverlay;               /* worlds 0 .. noverlay - 1 are drawn too (the reference draws 32) */
+  int32_t shadows;                /* 1: one shadow ray per lit pixel toward the directional light */
+  int32_t brute;                  /* measurement: 1 casts every ray against every geom, without the tile cull */
+  unsigned char* rgb;
+  float* depth;
+  int32_t* seg;
+} B2RenderArgs;
+int b2_render(b2_sim* sim, const B2RenderArgs* args, void* cuda_stream);
+
 /* Diagnostics (synchronises `cuda_stream`). */
 int b2_stats(b2_sim* sim, void* cuda_stream, B2Stats* out);
 /* Number of kernels this library has launched for `sim` since creation. */

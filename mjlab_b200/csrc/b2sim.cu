@@ -18,6 +18,7 @@
 #include "b2_obshist.cuh"
 #include "b2_events.cuh"
 #include "b2_nanguard.cuh"
+#include "b2_render.cuh"
 
 static thread_local std::string g_err;
 static int fail(const std::string& msg) {
@@ -76,6 +77,9 @@ struct b2_sim {
   int guard_on = 0, guard_buffer = 0;
   B2Guard guard = {};
   std::vector<void*> host_allocs;
+  // b2_render: the drawable geoms, listed at the first call
+  bool render_planned = false;
+  B2RenderPlan render_plan = {};
 };
 
 static int pad4(int n) { return (n + 3) & ~3; }
@@ -1531,6 +1535,75 @@ int b2_step_host(b2_sim* s, const float* ctrl_host, int nsteps, float* qpos_host
   if (qvel_host)
     CUDA_OK(cudaMemcpy2DAsync(qvel_host, sizeof(float) * m.nv, d.qvel.p, sizeof(float) * d.qvel.stride,
                               sizeof(float) * m.nv, s->nworld, cudaMemcpyDeviceToHost, st));
+  return 0;
+}
+
+// The drawable geoms (b2_render.cuh: B2RenderPlan), from the model's tables on the device.
+static int render_plan(b2_sim* s) {
+  const DevModel& m = s->hm;
+  auto fetch = [](const int* p, int n) {
+    std::vector<int> v((size_t)std::max(n, 0));
+    if (n > 0 && cudaMemcpy(v.data(), p, sizeof(int) * n, cudaMemcpyDeviceToHost) != cudaSuccess) v.clear();
+    return v;
+  };
+  const std::vector<int> type = fetch(m.geom_type, m.ngeom), body = fetch(m.geom_bodyid, m.ngeom);
+  const std::vector<int> parent = fetch(m.body_parentid, m.nbody), dofnum = fetch(m.body_dofnum, m.nbody);
+  const std::vector<int> sgeom = fetch(m.static_geom, m.nstatic), fgeom = fetch(m.fixed_geom, m.nfixed);
+  if ((int)type.size() != m.ngeom || (int)body.size() != m.ngeom || (int)parent.size() != m.nbody ||
+      (int)dofnum.size() != m.nbody || (int)sgeom.size() != m.nstatic || (int)fgeom.size() != m.nfixed)
+    return fail("b2_render: reading the model's tables failed");
+  std::vector<char> welded(m.nbody, 1);  // bodies are numbered parents first
+  for (int b = 1; b < m.nbody; b++) welded[b] = dofnum[b] == 0 && welded[parent[b]];
+  std::vector<int> pose(m.ngeom, -1), stat, dyn;
+  for (int k = 0; k < m.nstatic; k++) pose[sgeom[k]] = k;
+  for (int f = 0; f < m.nfixed; f++) pose[fgeom[f]] = -2 - f;
+  for (int g = 0; g < m.ngeom; g++) {
+    if (type[g] == G_MESH) continue;
+    if (welded[body[g]]) { stat.push_back(g); stat.push_back(pose[g]); }
+    else dyn.push_back(g);
+  }
+  B2RenderPlan& P = s->render_plan;
+  P.nstat = (int)stat.size() / 2;
+  P.ndyn = (int)dyn.size();
+  if (dev_upload<int>(s, stat, &P.stat) || dev_upload<int>(s, dyn, &P.dyn)) return 1;
+  s->render_planned = true;
+  return 0;
+}
+
+int b2_render(b2_sim* s, const B2RenderArgs* a, void* stream) {
+  if (!s || !a) return fail("b2_render: bad arguments");
+  if (a->width < 1 || a->width > 4096 || a->height < 1 || a->height > 4096)
+    return fail("b2_render: width and height must lie in 1..4096");
+  if (a->env_idx < 0 || a->env_idx >= s->nworld) return fail("b2_render: env_idx outside [0, nworld)");
+  if (a->noverlay < 0) return fail("b2_render: noverlay must be >= 0");
+  if (a->track_body < -1 || a->track_body >= s->hm.nbody) return fail("b2_render: track_body outside [-1, nbody)");
+  if (!a->rgb) return fail("b2_render: rgb is null");
+  DeviceGuard guard(s->device);
+  if (!s->render_planned && render_plan(s)) return 1;
+  const B2RenderPlan& P = s->render_plan;
+  B2RenderFrame F = {};
+  F.width = a->width; F.height = a->height;
+  F.ntx = (a->width + B2R_TILE - 1) / B2R_TILE;
+  const int nty = (a->height + B2R_TILE - 1) / B2R_TILE;
+  F.env_idx = a->env_idx;
+  F.noverlay = std::min(a->noverlay, s->nworld);
+  const int nworlds = F.noverlay + (a->env_idx >= F.noverlay ? 1 : 0);
+  F.nitem = P.nstat + nworlds * P.ndyn;
+  F.track_body = a->track_body;
+  F.shadows = a->shadows != 0; F.brute = a->brute != 0;
+  for (int k = 0; k < 3; k++) F.lookat[k] = a->lookat[k];
+  F.distance = a->distance;
+  const double deg = 3.14159265358979323846 / 180.0, az = a->azimuth * deg, el = a->elevation * deg;
+  const double f[3] = {std::cos(el) * std::cos(az), std::cos(el) * std::sin(az), std::sin(el)};
+  const double r[3] = {std::sin(az), -std::cos(az), 0.0};  // f x z, normalised
+  const double u[3] = {r[1] * f[2] - r[2] * f[1], r[2] * f[0] - r[0] * f[2], r[0] * f[1] - r[1] * f[0]};
+  for (int k = 0; k < 3; k++) { F.fwd[k] = (float)f[k]; F.right[k] = (float)r[k]; F.up[k] = (float)u[k]; }
+  F.tan_y = (float)std::tan(22.5 * deg);
+  F.tan_x = (float)(std::tan(22.5 * deg) * a->width / a->height);
+  F.rgb = a->rgb; F.depth = a->depth; F.seg = a->seg;
+  b2_render_kernel<<<F.ntx * nty, B2R_TILE * B2R_TILE, 0, (cudaStream_t)stream>>>(s->hm, s->hd, P, F);
+  s->launches++;
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 

@@ -29,6 +29,7 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass, field
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -39,6 +40,7 @@ from mjlab_b200.envs.events import (RESET_STATE_TERMS, ApplyExternalForceTorqueC
 from mjlab_b200.envs.motion import MotionClip
 from mjlab_b200.envs.noise import TaskNoise, tracking_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
+from mjlab_b200.render import RENDER_MODES, ViewerConfig, check_render_mode, env_render, env_renderer, task_viewer
 from mjlab_b200.envs.velocity_env import _resolve
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg, native
 
@@ -162,6 +164,9 @@ class TrackingEnvCfg:
   observations: ObservationsCfg = field(default_factory=ObservationsCfg)
   # randomize_field events (envs/events.py), run after the task's startup randomisation (startup_events)
   events: EventsCfg = field(default_factory=EventsCfg)
+  # the camera of env.render() with render_mode="rgb_array" (tracking_env_cfg.py:45-52; the robot's cfg names the body,
+  # tracking_task_cfg sets it)
+  viewer: ViewerConfig = field(default_factory=task_viewer)
 
   def __post_init__(self):
     self.check()
@@ -219,7 +224,9 @@ def tracking_task_cfg(name: str, **overrides) -> TrackingEnvCfg:
   `motion_file` override (without one the env runs the synthetic clip)."""
   if name not in TRACKING_TASKS:
     raise ValueError(f"unknown tracking task {name!r}; known: {', '.join(TRACKING_TASKS)}")
-  return TrackingEnvCfg(**{"episode_logs": True, **TRACKING_TASKS[name], **overrides})
+  # (the G1's camera override: tracking/config/g1/flat_env_cfg.py:54)
+  return TrackingEnvCfg(**{"episode_logs": True, "viewer": task_viewer(body_name="torso_link"), **TRACKING_TASKS[name],
+                           **overrides})
 
 
 def quat_inv(q):
@@ -255,7 +262,11 @@ def rot6(q):
 
 
 class TrackingFlatEnv:
-  def __init__(self, cfg: TrackingEnvCfg, device: str = "cuda:0", model=None, native_mdp: bool = True):
+  metadata = {"render_modes": RENDER_MODES}
+
+  def __init__(self, cfg: TrackingEnvCfg, device: str = "cuda:0", model=None, native_mdp: bool = True,
+               render_mode: str | None = None):
+    check_render_mode(render_mode)
     self.cfg, self.device = cfg, device
     self.native_mdp = native_mdp  # fused CUDA kernels (csrc/b2_trackenv.cuh) or the torch reference below
     self.model = m = model if model is not None else load_compiled("g1_tracking_flat")
@@ -326,6 +337,9 @@ class TrackingFlatEnv:
     self._init_task()
     self._graph = None
     self.reset()
+    self.render_mode = render_mode
+    self.metadata = {**self.metadata, "render_fps": 1.0 / self.step_dt}
+    self._offline_renderer = env_renderer(self.sim, cfg.viewer, render_mode)
 
   # -- helpers -------------------------------------------------------------------------------------
   def _rand(self, *shape):
@@ -814,5 +828,12 @@ class TrackingFlatEnv:
     self.events.step_interval_state()  # the interval push and wrench terms, after the observations
     return out["policy"], reward, terminated, truncated, self._extras(out["critic"])
 
+  def render(self) -> np.ndarray | None:
+    """The reference's ``env.render()``: None with ``render_mode=None``, else an (height, width, 3) uint8 frame of
+    ``cfg.viewer``'s camera, drawn on the GPU after the last step."""
+    return env_render(self._offline_renderer)
+
   def close(self):
+    if self._offline_renderer is not None:
+      self._offline_renderer.close()
     self.sim.close()

@@ -24,6 +24,7 @@ from mjlab_b200.envs import events as evm
 from mjlab_b200.envs.events import Events, EventsCfg, PushBySettingVelocityCfg, RandomizeFieldCfg
 from mjlab_b200.envs.noise import TaskNoise, velocity_defaults
 from mjlab_b200.envs.obs_history import Observations, ObservationsCfg
+from mjlab_b200.render import RENDER_MODES, ViewerConfig, check_render_mode, env_render, env_renderer, task_viewer
 from mjlab_b200.sim import MujocoCfg, Simulation, SimulationCfg
 
 
@@ -140,6 +141,9 @@ class VelocityEnvCfg:
   # event terms (envs/events.py), run after the startup foot friction of friction_range: randomize_field, and the
   # state terms push_by_setting_velocity (needs push_vel=None) and apply_external_force_torque
   events: EventsCfg = field(default_factory=EventsCfg)
+  # the camera of env.render() with render_mode="rgb_array" (velocity_env_cfg.py:41-48; the robot's cfg names the body,
+  # velocity_task_cfg sets it)
+  viewer: ViewerConfig = field(default_factory=task_viewer)
 
   def __post_init__(self):
     self.check()
@@ -173,6 +177,10 @@ VELOCITY_TASKS = {
 }
 
 
+# the robots' camera overrides (config/g1/rough_env_cfg.py:71, config/go1/rough_env_cfg.py:46-48)
+VIEWERS = {"g1": dict(body_name="torso_link"), "go1": dict(body_name="trunk", distance=1.5, elevation=-10.0)}
+
+
 def velocity_task_cfg(name: str, **overrides) -> VelocityEnvCfg:
   """The VelocityEnvCfg of one of the reference's velocity tasks by its registered name, with `overrides` (any
   VelocityEnvCfg field, e.g. num_envs) on top."""
@@ -180,6 +188,7 @@ def velocity_task_cfg(name: str, **overrides) -> VelocityEnvCfg:
     raise ValueError(f"unknown velocity task {name!r}; known: {', '.join(VELOCITY_TASKS)}")
   preset = dict(VELOCITY_TASKS[name])
   preset["posture_std"] = dict(preset["posture_std"])
+  preset["viewer"] = task_viewer(**VIEWERS[preset["robot"]])
   return VelocityEnvCfg(**{**preset, **overrides})
 
 
@@ -221,7 +230,11 @@ def quat_rotate_inverse(q: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
 
 
 class VelocityFlatEnv:
-  def __init__(self, cfg: VelocityEnvCfg, device: str = "cuda:0", model=None, native_mdp: bool = True):
+  metadata = {"render_modes": RENDER_MODES}
+
+  def __init__(self, cfg: VelocityEnvCfg, device: str = "cuda:0", model=None, native_mdp: bool = True,
+               render_mode: str | None = None):
+    check_render_mode(render_mode)
     self.cfg = cfg
     self.device = device
     zoo = g1 if cfg.robot == "g1" else go1
@@ -308,6 +321,9 @@ class VelocityFlatEnv:
     if self.native_mdp:
       self._init_native()
     self._reset_all(curriculum=False)  # no episode has ended yet: the initial levels stand
+    self.render_mode = render_mode
+    self.metadata = {**self.metadata, "render_fps": 1.0 / self.step_dt}
+    self._offline_renderer = env_renderer(self.sim, cfg.viewer, render_mode)
 
   # -- helpers -----------------------------------------------------------------------------------
   def _rand(self, *shape):
@@ -836,5 +852,12 @@ class VelocityFlatEnv:
     self.events.step_interval_state()  # the interval push and wrench terms, after the observations
     return out["policy"], reward, terminated, truncated, {"critic": out["critic"]}
 
+  def render(self) -> np.ndarray | None:
+    """The reference's ``env.render()``: None with ``render_mode=None``, else an (height, width, 3) uint8 frame of
+    ``cfg.viewer``'s camera, drawn on the GPU after the last step."""
+    return env_render(self._offline_renderer)
+
   def close(self):
+    if self._offline_renderer is not None:
+      self._offline_renderer.close()
     self.sim.close()

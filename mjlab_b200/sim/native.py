@@ -188,6 +188,13 @@ class B2EventArgs(ctypes.Structure):
 NAN_GUARD_ON = 1  # B2_NAN_GUARD_ON: b2_nan_guard's flag that arms the guard
 
 
+class B2RenderArgs(ctypes.Structure):
+  _fields_ = ([(n, ctypes.c_int32) for n in ("width", "height")] + [("lookat", ctypes.c_float * 3)]
+              + [("track_body", ctypes.c_int32)] + [(n, ctypes.c_float) for n in ("distance", "azimuth", "elevation")]
+              + [(n, ctypes.c_int32) for n in ("env_idx", "noverlay", "shadows", "brute")]
+              + [(n, ctypes.c_void_p) for n in ("rgb", "depth", "seg")])
+
+
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
 
 
@@ -250,6 +257,7 @@ def bind(L: ctypes.CDLL) -> ctypes.CDLL:
     "b2_nan_guard": ([vp, ci, ci, ci], ci),
     "b2_nan_guard_word": ([vp], vp),
     "b2_nan_guard_read": ([vp, vp, P(ctypes.c_int64), vp, vp], ci),
+    "b2_render": ([vp, P(B2RenderArgs), vp], ci),
     "b2_stats": ([vp, vp, P(B2Stats)], ci),
     "b2_launch_count": ([vp], ctypes.c_int64),
     "b2_algorithmic_bytes": ([vp, vp, P(cd), P(cd)], ci),
