@@ -511,7 +511,20 @@ int b2_nan_guard_read(b2_sim* sim, void* cuda_stream, int64_t* detected, float* 
  *         written).
  * Shading and its constants: DESIGN.md §4.  The first call on a sim builds the list of drawable geoms (it synchronises
  * the device: not capturable); later calls only launch.  Refused: a size outside 1..4096, env_idx outside
- * [0, nworld), noverlay < 0, track_body outside [-1, nbody), a null rgb. */
+ * [0, nworld), noverlay < 0, track_body outside [-1, nbody), a null rgb.
+ *
+ * Decoration (the debug visualisers: command arrows, a ghost of the robot), one translucent layer over the scene; zero
+ * fields mean none.  The nearest decoration item the ray enters before the scene's hit is shaded without shadows and
+ * blended, byte = floor(255 (a c_d + (1 - a) c_o) + 1/2), over the scene's colour c_o; decoration casts no shadow and
+ * is not in depth or seg.  A frame with decoration is two launches: the scene, with the outputs a frame without
+ * decoration has, then the decoration over the pixels it covers.
+ *   decor      device array of ndecor arrow records of 12 floats: from[3], to[3], width w, rgba[4], padding.  An
+ *              arrow is a cylinder shaft of radius w with flat caps and a solid cone head of base radius 2w, length
+ *              min(L/2, 4w) and apex at `to` (L = |to - from|); not drawn when L < 1e-6 or alpha is 0.  Refused:
+ *              ndecor outside [0, 64], a null decor with ndecor > 0.
+ *   ghost_xpos, ghost_xmat  device geom poses [ngeom][3], [ngeom][9] of one configuration of this model (null: no
+ *              ghost); the drawable geoms of bodies not welded to the world are drawn there in ghost_rgba, with world
+ *              env_idx's sizes.  Refused: one of the two null, ghost_rgba outside [0, 1] or not finite. */
 typedef struct B2RenderArgs {
   int32_t width, height;          /* pixels, 1..4096 */
   float lookat[3];                /* camera target when track_body is -1 */
@@ -524,6 +537,11 @@ typedef struct B2RenderArgs {
   unsigned char* rgb;
   float* depth;
   int32_t* seg;
+  const float* decor;             /* [ndecor][12] arrow records (device), or null */
+  int32_t ndecor;
+  const float* ghost_xpos;        /* [ngeom][3] (device), or null: no ghost */
+  const float* ghost_xmat;        /* [ngeom][9] (device) */
+  float ghost_rgba[4];
 } B2RenderArgs;
 int b2_render(b2_sim* sim, const B2RenderArgs* args, void* cuda_stream);
 

@@ -13,12 +13,22 @@
 //
 // Conventions (tests/test_render.py reproduces them in fp64): a solid geom is hit where the ray enters it (a ray that
 // starts inside sees nothing of it), a plane or height-field surface from either side.  Constants: DESIGN.md §4.
+//
+// Decoration (the debug visualisers' overlay, tests/test_render_debug_vis.py reproduces it in fp64): a ghost of the
+// dynamic geoms at other poses (ghost_xpos / ghost_xmat, sizes of world env_idx, one colour) and arrows (a cylinder
+// shaft of radius w and a cone head of base radius 2w and length min(L/2, 4w), apex at `to`).  Decoration items enter
+// the tile list after the scene's, so the scene's part of every loop is unchanged.  They are one translucent layer:
+// the nearest decoration entry in front of the opaque hit, shaded without shadows, is blended over the opaque colour;
+// it casts no shadow and is not in depth or seg.  A frame with decoration is two launches: the scene-only instance of
+// the kernel, then the decoration instance, which writes only the pixels decoration covers.
 #pragma once
 #include "b2_types.h"
 
 #define B2R_TILE 16
 #define B2R_LIST 2048  // tile list capacity (items)
 #define B2R_INF 3.0e38f
+#define B2R_MAXDECOR 64  // arrows per frame
+#define B2R_DECOR 12     // floats per arrow record: from[3], to[3], width, rgba[4], padding
 
 // The items' static part, built once per sim (b2_render): static geoms with their pose source, and the dynamic geoms.
 struct B2RenderPlan {
@@ -39,6 +49,12 @@ struct B2RenderFrame {
   unsigned char* rgb;
   float* depth;
   int* seg;
+  // decoration: items nitem .. nitem + ndeco - 1 of the cull; the first nghost are the ghost of P.dyn, then the arrows
+  int ndeco, nghost;
+  const float* decor;              // [ndeco - nghost][B2R_DECOR]
+  const float* ghost_xpos;         // [ngeom][3]
+  const float* ghost_xmat;         // [ngeom][9]
+  float ghost_rgba[4];
 };
 
 // light: unit direction toward the light; intensity = AMBIENT + DIFFUSE max(0, n.L) (0 when shadowed) + HEAD max(0, -n.d)
@@ -293,11 +309,158 @@ __device__ __forceinline__ void b2r_dir(const B2RenderFrame& F, float x, float y
   for (int k = 0; k < 3; k++) dir[k] = F.fwd[k] + a * F.right[k] + b * F.up[k];
 }
 
+// ---- decoration items
+
+// Ghost item j < F.nghost: the dynamic geom P.dyn[j] at the ghost's pose, with world env_idx's size and bound.
+__device__ __forceinline__ B2RItem b2r_ghost(const DevModel& m, const B2RenderPlan& P, const B2RenderFrame& F, int j) {
+  B2RItem it;
+  it.world = F.env_idx; it.geom = P.dyn[j];
+  it.pos = F.ghost_xpos + 3 * it.geom; it.mat = F.ghost_xmat + 9 * it.geom;
+  it.type = m.geom_type[it.geom];
+  return it;
+}
+
+// An arrow record's unit axis, length L and head length h; false when it is not drawn (L < 1e-6 or alpha 0).
+__device__ __forceinline__ bool b2r_arrow_axis(const float* a, float* ax, float& L, float& h) {
+  for (int k = 0; k < 3; k++) ax[k] = a[3 + k] - a[k];
+  L = sqrtf(ax[0] * ax[0] + ax[1] * ax[1] + ax[2] * ax[2]);
+  if (!(L >= 1e-6f) || a[10] == 0.f) return false;
+  const float inv = 1.f / L;
+  for (int k = 0; k < 3; k++) ax[k] *= inv;
+  h = fminf(0.5f * L, 4.f * a[6]);
+  return true;
+}
+
+// Bounding sphere (c, r) of decoration item j; false when the item is not drawn.
+__device__ __forceinline__ bool b2r_deco_bound(const DevModel& m, const B2RenderPlan& P, const B2RenderFrame& F, int j,
+                                               float* c, float& r) {
+  if (j < F.nghost) {
+    const B2RItem it = b2r_ghost(m, P, F, j);
+    for (int k = 0; k < 3; k++) c[k] = it.pos[k];
+    r = b2r_radius(m, it);
+    return true;
+  }
+  const float* a = F.decor + B2R_DECOR * (j - F.nghost);
+  float ax[3], L, h;
+  if (!b2r_arrow_axis(a, ax, L, h)) return false;
+  for (int k = 0; k < 3; k++) c[k] = 0.5f * (a[k] + a[3 + k]);
+  r = sqrtf(0.25f * L * L + 4.f * a[6] * a[6]);
+  return true;
+}
+
+// Entry t in (0, tmax) of the ray ow + t dw (d unit) into the arrow record a, or B2R_INF; n: world normal there (not
+// normalised).  In the arrow's frame (z along the axis, `from` at the origin) the shaft is |xy| <= w, 0 <= z <= L - h,
+// and the head is the solid cone of apex (0, 0, L) and base radius 2w at z = L - h.
+__device__ float b2r_arrow(const float* a, const float* ow, const float* dw, float tmax, float* n) {
+  float ez[3], L, h;
+  if (!b2r_arrow_axis(a, ez, L, h)) return B2R_INF;
+  const float w = a[6];
+  float ex[3], ey[3];
+  {
+    const float hx = fabsf(ez[0]) < 0.9f ? 1.f : 0.f, hy = 1.f - hx, p = hx * ez[0] + hy * ez[1];
+    ex[0] = hx - p * ez[0]; ex[1] = hy - p * ez[1]; ex[2] = -p * ez[2];
+    const float inv = rsqrtf(ex[0] * ex[0] + ex[1] * ex[1] + ex[2] * ex[2]);
+    for (int k = 0; k < 3; k++) ex[k] *= inv;
+    ey[0] = ez[1] * ex[2] - ez[2] * ex[1]; ey[1] = ez[2] * ex[0] - ez[0] * ex[2]; ey[2] = ez[0] * ex[1] - ez[1] * ex[0];
+  }
+  const float v[3] = {ow[0] - a[0], ow[1] - a[1], ow[2] - a[2]};
+  const float o[3] = {ex[0] * v[0] + ex[1] * v[1] + ex[2] * v[2], ey[0] * v[0] + ey[1] * v[1] + ey[2] * v[2],
+                      ez[0] * v[0] + ez[1] * v[1] + ez[2] * v[2]};
+  const float d[3] = {ex[0] * dw[0] + ex[1] * dw[1] + ex[2] * dw[2], ey[0] * dw[0] + ey[1] * dw[1] + ey[2] * dw[2],
+                      ez[0] * dw[0] + ez[1] * dw[1] + ez[2] * dw[2]};
+  float t = B2R_INF, nl[3] = {0.f, 0.f, 0.f}, lo, hi, zl, zh;
+  // shaft: a cylinder with flat caps
+  if (b2r_tube(o, d, w, lo, hi)) {
+    b2r_slab(o[2] - 0.5f * (L - h), d[2], 0.5f * (L - h), zl, zh);
+    const float e = fmaxf(lo, zl);
+    if (e <= fminf(hi, zh) && e > 0.f) {
+      t = e;
+      if (lo >= zl) { nl[0] = o[0] + t * d[0]; nl[1] = o[1] + t * d[1]; }
+      else nl[2] = d[2] > 0.f ? -1.f : 1.f;
+    }
+  }
+  // head: the ray's interval (lo, hi) in the cone's nappe z <= L, clipped to L - h <= z <= L
+  {
+    const float k2 = (2.f * w / h) * (2.f * w / h), qz = o[2] - L;
+    const float A = d[0] * d[0] + d[1] * d[1] - k2 * d[2] * d[2];
+    const float B = o[0] * d[0] + o[1] * d[1] - k2 * qz * d[2];
+    const float C = o[0] * o[0] + o[1] * o[1] - k2 * qz * qz;
+    const float disc = B * B - A * C;
+    float r1 = B2R_INF, r2 = B2R_INF;
+    bool v1 = false, v2 = false;
+    if (A != 0.f && disc >= 0.f) {
+      const float sq = sqrtf(disc), x1 = (-B - sq) / A, x2 = (-B + sq) / A;
+      r1 = fminf(x1, x2); r2 = fmaxf(x1, x2);
+      v1 = qz + r1 * d[2] <= 0.f; v2 = qz + r2 * d[2] <= 0.f;
+    } else if (A == 0.f && B != 0.f) {
+      r1 = -0.5f * C / B;
+      v1 = qz + r1 * d[2] <= 0.f;
+    }
+    lo = B2R_INF; hi = -B2R_INF;
+    if (v1 && v2) { lo = r1; hi = r2; }
+    else if (v1 || v2) {  // the ray leaves the nappe toward +z, or enters it toward -z and stays
+      const float r = v1 ? r1 : r2;
+      if (d[2] < 0.f) { lo = r; hi = B2R_INF; }
+      else { lo = -B2R_INF; hi = r; }
+    }
+    b2r_slab(o[2] - (L - 0.5f * h), d[2], 0.5f * h, zl, zh);
+    const float e = fmaxf(lo, zl);
+    if (e <= fminf(hi, zh) && e > 0.f && e < t) {
+      t = e;
+      if (lo >= zl) { nl[0] = o[0] + t * d[0]; nl[1] = o[1] + t * d[1]; nl[2] = -k2 * (qz + t * d[2]); }
+      else { nl[0] = 0.f; nl[1] = 0.f; nl[2] = d[2] > 0.f ? -1.f : 1.f; }
+    }
+  }
+  if (!(t < tmax)) return B2R_INF;
+  for (int k = 0; k < 3; k++) n[k] = ex[k] * nl[0] + ey[k] * nl[1] + ez[k] * nl[2];
+  return t;
+}
+
+// The decoration pass of one ray o + t dir (dir unit): the nearest decoration item among entries first .. last - 1 of
+// the tile list (all: every item) entered before `best`, or -1; dc: its shaded, clamped colour and its alpha.  The
+// decoration instance of b2_render_kernel.
+__device__ __forceinline__ int b2r_decorate(const DevModel& m, const B2RenderPlan& P, const B2RenderFrame& F,
+                                         const int* list, int first, int last, bool all, const float* o,
+                                         const float* dir, float best, float* dc) {
+  int deco = -1;
+  float dbest = best, dn[3];
+  for (int j = first; j < last; j++) {
+    const int k = all ? j : list[j] - F.nitem;
+    float nn[3], t;
+    if (k < F.nghost) {
+      const B2RItem it = b2r_ghost(m, P, F, k);
+      if (!b2r_near(o, dir, it.pos, b2r_radius(m, it), dbest)) continue;
+      int ck;
+      t = b2r_hit(m, it, o, dir, 0.f, dbest, nn, &ck);
+    } else {
+      t = b2r_arrow(F.decor + B2R_DECOR * (k - F.nghost), o, dir, dbest, nn);
+    }
+    if (t < dbest) { dbest = t; deco = k; dn[0] = nn[0]; dn[1] = nn[1]; dn[2] = nn[2]; }
+  }
+  if (deco >= 0) {
+    const float inv = rsqrtf(dn[0] * dn[0] + dn[1] * dn[1] + dn[2] * dn[2]);
+    const float sg = (dn[0] * dir[0] + dn[1] * dir[1] + dn[2] * dir[2]) > 0.f ? -inv : inv;
+    for (int k = 0; k < 3; k++) dn[k] *= sg;
+    const float light = B2R_AMBIENT + B2R_DIFFUSE * fmaxf(0.f, dn[0] * B2R_LX + dn[1] * B2R_LY + dn[2] * B2R_LZ) +
+                        B2R_HEAD * fmaxf(0.f, -(dn[0] * dir[0] + dn[1] * dir[1] + dn[2] * dir[2]));
+    const float* c = deco < F.nghost ? F.ghost_rgba : F.decor + B2R_DECOR * (deco - F.nghost) + 7;
+    for (int k = 0; k < 3; k++) dc[k] = fminf(fmaxf(c[k] * light, 0.f), 1.f);
+    dc[3] = c[3];
+  }
+  return deco;
+}
+
+// DECO = false draws the scene: every pixel's rgb, depth and seg.  DECO = true runs after it on frames with decoration
+// and writes only the rgb of the pixels a decoration item covers, blended over the scene's colour, which it recomputes
+// for them.  So the scene's outputs come from the same instance with decoration or without, bit for bit (two
+// instances of the scene's code need not round alike: the compiler contracts their arithmetic independently), and
+// the scene-only instance keeps its register budget.
+template <bool DECO>
 __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel m, DevData d, B2RenderPlan P,
                                                                         B2RenderFrame F) {
   __shared__ int list[B2R_LIST];
-  __shared__ int warp_n[B2R_TILE * B2R_TILE / 32];
-  __shared__ int nlist, overflow;
+  __shared__ int warp_n[B2R_TILE * B2R_TILE / 32], warp_s[B2R_TILE * B2R_TILE / 32];
+  __shared__ int nlist, nscene, overflow;  // nscene: the list's scene items, before its decoration items
   __shared__ float eye[3];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int tile_x = blockIdx.x % F.ntx, tile_y = blockIdx.x / F.ntx;
@@ -306,7 +469,7 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
     const float* c = F.lookat;
     if (F.track_body >= 0) c = d.subtree_com.p + (size_t)F.env_idx * d.subtree_com.stride + 3 * F.track_body;
     for (int k = 0; k < 3; k++) eye[k] = c[k] - F.distance * F.fwd[k];
-    nlist = 0;
+    nlist = nscene = 0;
     overflow = F.brute;
   }
   __syncthreads();
@@ -328,24 +491,28 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
         pl[e][0] = nx * inv; pl[e][1] = ny * inv; pl[e][2] = nz * inv;
       }
     }
-    for (int base = 0; base < F.nitem; base += B2R_TILE * B2R_TILE) {
+    // the scene's items 0 .. nitem - 1, then the decoration's nitem .. nitem + ndeco - 1 (list entry nitem + j)
+    const int ncull = DECO ? F.nitem + F.ndeco : F.nitem;
+    for (int base = 0; base < ncull; base += B2R_TILE * B2R_TILE) {
       const int i = base + tid;
       bool keep = false;
+      float c[3], r = 0.f;
       if (i < F.nitem) {
         const B2RItem it = b2r_item(m, d, P, F, i);
-        if (b2r_drawn(m, it)) {
-          const float r = b2r_radius(m, it);
-          keep = true;
-          if (r < B2R_INF) {
-            const float v[3] = {it.pos[0] - o[0], it.pos[1] - o[1], it.pos[2] - o[2]};
-            const float rr = r * 1.001f + 1e-4f * (1.f + sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
-            keep = v[0] * F.fwd[0] + v[1] * F.fwd[1] + v[2] * F.fwd[2] >= -rr;
-            for (int e = 0; e < 4; e++) keep &= pl[e][0] * v[0] + pl[e][1] * v[1] + pl[e][2] * v[2] >= -rr;
-          }
-        }
+        keep = b2r_drawn(m, it);
+        if (keep) { r = b2r_radius(m, it); c[0] = it.pos[0]; c[1] = it.pos[1]; c[2] = it.pos[2]; }
+      } else if (DECO && i < ncull) {
+        keep = b2r_deco_bound(m, P, F, i - F.nitem, c, r);
+      }
+      if (keep && r < B2R_INF) {
+        const float v[3] = {c[0] - o[0], c[1] - o[1], c[2] - o[2]};
+        const float rr = r * 1.001f + 1e-4f * (1.f + sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]));
+        keep = v[0] * F.fwd[0] + v[1] * F.fwd[1] + v[2] * F.fwd[2] >= -rr;
+        for (int e = 0; e < 4; e++) keep &= pl[e][0] * v[0] + pl[e][1] * v[1] + pl[e][2] * v[2] >= -rr;
       }
       const unsigned bal = __ballot_sync(0xffffffffu, keep);
-      if (lane == 0) warp_n[warp] = __popc(bal);
+      const unsigned bal_scene = DECO ? __ballot_sync(0xffffffffu, keep && i < F.nitem) : bal;
+      if (lane == 0) { warp_n[warp] = __popc(bal); warp_s[warp] = __popc(bal_scene); }
       __syncthreads();
       int off = nlist;
       for (int w = 0; w < warp; w++) off += warp_n[w];
@@ -355,7 +522,8 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
         else overflow = 1;
       }
       __syncthreads();
-      if (tid == 0) for (int w = 0; w < B2R_TILE * B2R_TILE / 32; w++) nlist += warp_n[w];
+      if (tid == 0)
+        for (int w = 0; w < B2R_TILE * B2R_TILE / 32; w++) { nlist += warp_n[w]; nscene += warp_s[w]; }
       __syncthreads();
     }
   }
@@ -368,7 +536,7 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
     for (int k = 0; k < 3; k++) dir[k] *= inv;
   }
   const bool all = overflow != 0;
-  const int count = all ? F.nitem : nlist;
+  const int count = all ? F.nitem : nscene;
   float best = B2R_INF, n[3] = {0.f, 0.f, 1.f};
   int hit = -1, checker = 0;
   for (int j = 0; j < count; j++) {
@@ -381,11 +549,25 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
     const float t = b2r_hit(m, it, o, dir, 0.f, best, nn, &ck);
     if (t < best) { best = t; hit = i; checker = ck; n[0] = nn[0]; n[1] = nn[1]; n[2] = nn[2]; }
   }
+  const float L[3] = {B2R_LX, B2R_LY, B2R_LZ};
+  // ---- decoration: the nearest item entered before the opaque hit, shaded without shadows (dc: colour and alpha)
+  int deco = -1;
+  float dc[4];
+  if (DECO) {
+    deco = b2r_decorate(m, P, F, list, all ? 0 : nscene, all ? F.ndeco : nlist, all, o, dir, best, dc);
+    if (deco < 0) return;  // the scene instance drew this pixel
+  }
   const size_t pix = (size_t)py * F.width + px;
   if (hit < 0) {
-    F.rgb[3 * pix] = B2R_BG_R; F.rgb[3 * pix + 1] = B2R_BG_G; F.rgb[3 * pix + 2] = B2R_BG_B;
-    if (F.depth) F.depth[pix] = __int_as_float(0x7f800000);
-    if (F.seg) { F.seg[2 * pix] = -1; F.seg[2 * pix + 1] = -1; }
+    if (!DECO) {
+      F.rgb[3 * pix] = B2R_BG_R; F.rgb[3 * pix + 1] = B2R_BG_G; F.rgb[3 * pix + 2] = B2R_BG_B;
+      if (F.depth) F.depth[pix] = __int_as_float(0x7f800000);
+      if (F.seg) { F.seg[2 * pix] = -1; F.seg[2 * pix + 1] = -1; }
+    } else {
+      const float bg[3] = {B2R_BG_R / 255.f, B2R_BG_G / 255.f, B2R_BG_B / 255.f};
+      for (int k = 0; k < 3; k++)
+        F.rgb[3 * pix + k] = (unsigned char)((dc[3] * dc[k] + (1.f - dc[3]) * bg[k]) * 255.f + 0.5f);
+    }
     return;
   }
   const B2RItem hi = b2r_item(m, d, P, F, hit);
@@ -394,10 +576,9 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
     const float sg = (n[0] * dir[0] + n[1] * dir[1] + n[2] * dir[2]) > 0.f ? -inv : inv;  // toward the camera
     for (int k = 0; k < 3; k++) n[k] *= sg;
   }
-  const float L[3] = {B2R_LX, B2R_LY, B2R_LZ};
   float diff = fmaxf(0.f, n[0] * L[0] + n[1] * L[1] + n[2] * L[2]);
   if (F.shadows && diff > 0.f) {
-    // ---- shadow ray toward the light, against every item
+    // ---- shadow ray toward the light, against every scene item
     float p[3];
     for (int k = 0; k < 3; k++) p[k] = o[k] + best * dir[k] + B2R_SHADOW_EPS * n[k];
     for (int i = 0; i < F.nitem && diff > 0.f; i++) {
@@ -412,7 +593,14 @@ __global__ void __launch_bounds__(B2R_TILE * B2R_TILE) b2_render_kernel(DevModel
   float light = B2R_AMBIENT + B2R_DIFFUSE * diff + B2R_HEAD * head;
   if (hi.type == G_PLANE && checker) light *= B2R_CHECKER_DARK;
   const float* rgba = b2r_rgba(m, hi);
-  for (int k = 0; k < 3; k++) F.rgb[3 * pix + k] = (unsigned char)(fminf(fmaxf(rgba[k] * light, 0.f), 1.f) * 255.f + 0.5f);
-  if (F.depth) F.depth[pix] = best * (dir[0] * F.fwd[0] + dir[1] * F.fwd[1] + dir[2] * F.fwd[2]);
-  if (F.seg) { F.seg[2 * pix] = hi.world; F.seg[2 * pix + 1] = hi.geom; }
+  if (!DECO) {
+    for (int k = 0; k < 3; k++) F.rgb[3 * pix + k] = (unsigned char)(fminf(fmaxf(rgba[k] * light, 0.f), 1.f) * 255.f + 0.5f);
+    if (F.depth) F.depth[pix] = best * (dir[0] * F.fwd[0] + dir[1] * F.fwd[1] + dir[2] * F.fwd[2]);
+    if (F.seg) { F.seg[2 * pix] = hi.world; F.seg[2 * pix + 1] = hi.geom; }
+  } else {
+    for (int k = 0; k < 3; k++) {
+      const float co = fminf(fmaxf(rgba[k] * light, 0.f), 1.f);
+      F.rgb[3 * pix + k] = (unsigned char)((dc[3] * dc[k] + (1.f - dc[3]) * co) * 255.f + 0.5f);
+    }
+  }
 }

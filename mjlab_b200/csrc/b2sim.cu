@@ -1578,6 +1578,14 @@ int b2_render(b2_sim* s, const B2RenderArgs* a, void* stream) {
   if (a->noverlay < 0) return fail("b2_render: noverlay must be >= 0");
   if (a->track_body < -1 || a->track_body >= s->hm.nbody) return fail("b2_render: track_body outside [-1, nbody)");
   if (!a->rgb) return fail("b2_render: rgb is null");
+  if (a->ndecor < 0 || a->ndecor > B2R_MAXDECOR)
+    return fail("b2_render: ndecor " + std::to_string(a->ndecor) + " outside [0, " + std::to_string(B2R_MAXDECOR) + "]");
+  if (a->ndecor > 0 && !a->decor) return fail("b2_render: decor is null with ndecor > 0");
+  if (!a->ghost_xpos != !a->ghost_xmat) return fail("b2_render: ghost_xpos and ghost_xmat must both be set or both null");
+  if (a->ghost_xpos)
+    for (int k = 0; k < 4; k++)
+      if (!(a->ghost_rgba[k] >= 0.f && a->ghost_rgba[k] <= 1.f))
+        return fail("b2_render: ghost_rgba must lie in [0, 1]");
   DeviceGuard guard(s->device);
   if (!s->render_planned && render_plan(s)) return 1;
   const B2RenderPlan& P = s->render_plan;
@@ -1601,8 +1609,17 @@ int b2_render(b2_sim* s, const B2RenderArgs* a, void* stream) {
   F.tan_y = (float)std::tan(22.5 * deg);
   F.tan_x = (float)(std::tan(22.5 * deg) * a->width / a->height);
   F.rgb = a->rgb; F.depth = a->depth; F.seg = a->seg;
-  b2_render_kernel<<<F.ntx * nty, B2R_TILE * B2R_TILE, 0, (cudaStream_t)stream>>>(s->hm, s->hd, P, F);
+  F.nghost = a->ghost_xpos ? P.ndyn : 0;
+  F.ndeco = F.nghost + a->ndecor;
+  F.decor = a->decor; F.ghost_xpos = a->ghost_xpos; F.ghost_xmat = a->ghost_xmat;
+  for (int k = 0; k < 4; k++) F.ghost_rgba[k] = a->ghost_rgba[k];
+  // the scene, then (with decoration) the decoration over it: b2_render.cuh, b2_render_kernel
+  b2_render_kernel<false><<<F.ntx * nty, B2R_TILE * B2R_TILE, 0, (cudaStream_t)stream>>>(s->hm, s->hd, P, F);
   s->launches++;
+  if (F.ndeco > 0) {
+    b2_render_kernel<true><<<F.ntx * nty, B2R_TILE * B2R_TILE, 0, (cudaStream_t)stream>>>(s->hm, s->hd, P, F);
+    s->launches++;
+  }
   CUDA_OK(cudaGetLastError());
   return 0;
 }

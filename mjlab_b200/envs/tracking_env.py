@@ -167,6 +167,10 @@ class TrackingEnvCfg:
   # the camera of env.render() with render_mode="rgb_array" (tracking_env_cfg.py:45-52; the robot's cfg names the body,
   # tracking_task_cfg sets it)
   viewer: ViewerConfig = field(default_factory=task_viewer)
+  # the motion command's ghost in env.render() frames (commands.py:400-416): the robot posed at the clip's current
+  # frame of cfg.viewer.env_idx, drawn translucent in ghost_color (MotionCommandCfg.VizCfg, commands.py:436-439)
+  debug_vis: bool = False
+  ghost_color: tuple = (0.5, 0.7, 0.5, 0.5)
 
   def __post_init__(self):
     self.check()
@@ -221,7 +225,8 @@ def startup_events(cfg: TrackingEnvCfg) -> tuple:
 def tracking_task_cfg(name: str, **overrides) -> TrackingEnvCfg:
   """The TrackingEnvCfg of one of the reference's tracking tasks by its registered name, with `overrides` (any
   TrackingEnvCfg field) on top.  As in the reference, whose robot cfg leaves it empty, the clip comes in as the
-  `motion_file` override (without one the env runs the synthetic clip)."""
+  `motion_file` override (without one the env runs the synthetic clip).  The presets leave the motion's ghost off,
+  so their frames show the scene alone; the reference's tasks turn it on, which `debug_vis=True` does here."""
   if name not in TRACKING_TASKS:
     raise ValueError(f"unknown tracking task {name!r}; known: {', '.join(TRACKING_TASKS)}")
   # (the G1's camera override: tracking/config/g1/flat_env_cfg.py:54)
@@ -831,7 +836,24 @@ class TrackingFlatEnv:
   def render(self) -> np.ndarray | None:
     """The reference's ``env.render()``: None with ``render_mode=None``, else an (height, width, 3) uint8 frame of
     ``cfg.viewer``'s camera, drawn on the GPU after the last step."""
-    return env_render(self._offline_renderer)
+    return env_render(self._offline_renderer, self.update_visualizers if self.cfg.debug_vis else None)
+
+  def ghost_qpos(self, env_idx: int) -> torch.Tensor:
+    """(nq,) pose of the motion's current frame for one env (commands.py:410-414): the first tracked body's (the
+    pelvis's) position plus the env origin and its orientation as the free joint, the clip's joint positions."""
+    ix = self.robot.indexing
+    ts = self.time_steps[env_idx:env_idx + 1]
+    q = torch.zeros(self.nq, dtype=torch.float32, device=self.device)
+    q[ix.free_joint_q_adr[:3]] = self.motion["body_pos_w"][ts, 0][0] + self.env_origins[env_idx]
+    q[ix.free_joint_q_adr[3:7]] = self.motion["body_quat_w"][ts, 0][0]
+    q[ix.joint_q_adr] = self.motion["joint_pos"][ts][0]
+    return q
+
+  def update_visualizers(self, visualizer) -> None:
+    """The motion command's ghost for ``visualizer.env_idx`` (commands.py:400-416), built on the device."""
+    if visualizer.env_idx >= self.num_envs:
+      return
+    visualizer.add_ghost_mesh(self.ghost_qpos(visualizer.env_idx), self.cfg.ghost_color)
 
   def close(self):
     if self._offline_renderer is not None:

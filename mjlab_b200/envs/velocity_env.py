@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from mjlab_b200.asset_zoo import g1, go1, load_compiled
-from mjlab_b200.entity_data import EntityIndexing
+from mjlab_b200.entity_data import EntityIndexing, quat_apply
 from mjlab_b200.envs import events as evm
 from mjlab_b200.envs.events import Events, EventsCfg, PushBySettingVelocityCfg, RandomizeFieldCfg
 from mjlab_b200.envs.noise import TaskNoise, velocity_defaults
@@ -88,6 +88,16 @@ class VelocityCommandCfg:
   heading_control_stiffness: float = 0.5
   rel_standing_envs: float = 0.1
   resampling_time_range: tuple = (3.0, 8.0)
+  # the command's arrows in env.render() frames (velocity_command.py:106-177): commanded and actual planar velocity
+  # and yaw rate of cfg.viewer.env_idx, drawn viz.z_offset above the root and scaled by viz.scale
+  debug_vis: bool = False
+
+  @dataclass
+  class VizCfg:
+    z_offset: float = 0.2
+    scale: float = 0.75
+
+  viz: VizCfg = field(default_factory=VizCfg)
 
   def __post_init__(self):
     self.check()
@@ -183,7 +193,9 @@ VIEWERS = {"g1": dict(body_name="torso_link"), "go1": dict(body_name="trunk", di
 
 def velocity_task_cfg(name: str, **overrides) -> VelocityEnvCfg:
   """The VelocityEnvCfg of one of the reference's velocity tasks by its registered name, with `overrides` (any
-  VelocityEnvCfg field, e.g. num_envs) on top."""
+  VelocityEnvCfg field, e.g. num_envs) on top.  The presets leave the command's debug visualisation off, so their
+  frames show the scene alone; the reference's tasks turn it on, which `command=VelocityCommandCfg(debug_vis=True)`
+  does here."""
   if name not in VELOCITY_TASKS:
     raise ValueError(f"unknown velocity task {name!r}; known: {', '.join(VELOCITY_TASKS)}")
   preset = dict(VELOCITY_TASKS[name])
@@ -221,6 +233,22 @@ def _resolve(pattern_map: dict, names: list[str], default: float) -> list[float]
     else:
       out.append(default)
   return out
+
+
+# (rgba of the commanded and actual planar velocity and yaw rate arrows, velocity_command.py:146-177; width 0.015)
+VELOCITY_ARROW_COLORS = ((0.2, 0.2, 0.6, 0.6), (0.2, 0.6, 0.2, 0.6), (0.0, 0.6, 1.0, 0.7), (0.0, 1.0, 0.4, 0.7))
+VELOCITY_ARROW_WIDTH = 0.015
+
+
+def velocity_arrows(pos, quat, cmd, lin_vel_b, ang_vel_b, z_offset: float, scale: float) -> torch.Tensor:
+  """(4, 2, 3) world (from, to) of the command's arrows for one env (velocity_command.py:135-177): commanded and
+  actual planar velocity, commanded and actual yaw rate, from (0, 0, z_offset)·scale in the root frame."""
+  z = torch.zeros(4, 2, 3, dtype=pos.dtype, device=pos.device)
+  z[..., 2] = z_offset
+  z[0, 1, :2], z[2, 1, :2] = cmd[:2], lin_vel_b[:2]
+  z[1, 1, 2] += cmd[2]
+  z[3, 1, 2] += ang_vel_b[2]
+  return pos + quat_apply(quat.expand(8, 4), (z * scale).reshape(8, 3)).reshape(4, 2, 3)
 
 
 def quat_rotate_inverse(q: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
@@ -324,6 +352,7 @@ class VelocityFlatEnv:
     self.render_mode = render_mode
     self.metadata = {**self.metadata, "render_fps": 1.0 / self.step_dt}
     self._offline_renderer = env_renderer(self.sim, cfg.viewer, render_mode)
+    self._vis = None  # the debug visualisation's EntityData and arrow colours, made at its first frame
 
   # -- helpers -----------------------------------------------------------------------------------
   def _rand(self, *shape):
@@ -855,7 +884,29 @@ class VelocityFlatEnv:
   def render(self) -> np.ndarray | None:
     """The reference's ``env.render()``: None with ``render_mode=None``, else an (height, width, 3) uint8 frame of
     ``cfg.viewer``'s camera, drawn on the GPU after the last step."""
-    return env_render(self._offline_renderer)
+    return env_render(self._offline_renderer, self.update_visualizers if self.cfg.command.debug_vis else None)
+
+  def update_visualizers(self, visualizer) -> None:
+    """The velocity command's arrows for ``visualizer.env_idx`` (velocity_command.py:106-177), from the root link's
+    pose and body-frame velocity and the command, computed on the device.  A root at the world origin (an env not yet
+    placed) draws its arrows with alpha 0, i.e. not at all."""
+    e = visualizer.env_idx
+    if e >= self.num_envs:
+      return
+    if self._vis is None:
+      from mjlab_b200.entity_data import EntityData
+
+      ix = EntityIndexing.from_model(self.model, "robot", self.device)
+      colors = torch.tensor(VELOCITY_ARROW_COLORS, dtype=torch.float32, device=self.device)
+      self._vis = (EntityData(ix, self.sim.data, self.sim.model, self.device, self.num_envs), colors)
+    robot, colors = self._vis
+    pos = robot.root_link_pos_w[e]
+    viz = self.cfg.command.viz
+    ends = velocity_arrows(pos, robot.root_link_quat_w[e], self.command[e], robot.root_link_lin_vel_b[e],
+                           robot.root_link_ang_vel_b[e], viz.z_offset, viz.scale)
+    colors = torch.cat([colors[:, :3], colors[:, 3:] * (pos.norm() >= 1e-6)], dim=1)
+    for k in range(4):
+      visualizer.add_arrow(ends[k, 0], ends[k, 1], colors[k], width=VELOCITY_ARROW_WIDTH)
 
   def close(self):
     if self._offline_renderer is not None:

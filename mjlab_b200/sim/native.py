@@ -192,7 +192,11 @@ class B2RenderArgs(ctypes.Structure):
   _fields_ = ([(n, ctypes.c_int32) for n in ("width", "height")] + [("lookat", ctypes.c_float * 3)]
               + [("track_body", ctypes.c_int32)] + [(n, ctypes.c_float) for n in ("distance", "azimuth", "elevation")]
               + [(n, ctypes.c_int32) for n in ("env_idx", "noverlay", "shadows", "brute")]
-              + [(n, ctypes.c_void_p) for n in ("rgb", "depth", "seg")])
+              + [(n, ctypes.c_void_p) for n in ("rgb", "depth", "seg", "decor")] + [("ndecor", ctypes.c_int32)]
+              + [(n, ctypes.c_void_p) for n in ("ghost_xpos", "ghost_xmat")] + [("ghost_rgba", ctypes.c_float * 4)])
+
+
+RENDER_MAXDECOR, RENDER_DECOR = 64, 12  # B2R_MAXDECOR arrows per frame of B2R_DECOR floats (csrc/b2_render.cuh)
 
 
 START_UNIFORM, START_ADAPTIVE, START_FIRST = 0, 1, 2  # B2TrackEnvArgs.adaptive (B2_START_* of include/b2sim.h)
