@@ -4,7 +4,7 @@
 The motion: every joint swings sinusoidally about the KNEES_BENT keyframe, inside its soft limits (the legs only a
 little, so the feet stay near the ground), with the analytic joint velocity; the pelvis drifts forward, bobs and
 turns slowly.  Body poses and velocities come from one forward with one world per frame, as the reference's
-scripts/csv_to_npz.py does (set qpos / qvel, forward, read the link states).  `sim` may be any object with the `Simulation` interface (e.g. one on the host-emulated library)."""
+scripts/csv_to_npz.py does (`mjlab_b200.envs.motion.record_motion`: set qpos / qvel, forward, read the link states).  `sim` may be any object with the `Simulation` interface (e.g. one on the host-emulated library)."""
 
 from __future__ import annotations
 
@@ -13,28 +13,26 @@ import math
 import sys
 from pathlib import Path
 
-import numpy as np
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 
 from mjlab_b200.asset_zoo import load_compiled  # noqa: E402
-from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_apply_inverse, quat_mul  # noqa: E402
+from mjlab_b200.entity_data import EntityData, EntityIndexing, quat_mul  # noqa: E402
+from mjlab_b200.envs.motion import record_motion  # noqa: E402
 from mjlab_b200.sim import Simulation, SimulationCfg  # noqa: E402
 
 
-def make_clip(path, frames: int = 960, fps: float = 50.0, device: str = "cuda:0", sim=None, model=None) -> str:
-  m = model if model is not None else load_compiled("g1_tracking_flat")
-  if sim is None:
-    sim = Simulation(frames, SimulationCfg(), m, device)
+def motion_law(m, ix: EntityIndexing, soft_limits: torch.Tensor, frames: int, fps: float, device: str):
+  """The clip's root and joint states at ``frames`` samples ``1 / fps`` apart, float32: root position, root quaternion
+  (wxyz), root linear and angular velocity (world frame), joint positions and velocities (entity joint order).
+  ``soft_limits`` is the entity's ``[nu, 2]`` soft joint range."""
   dev = torch.device(device)
-  ix = EntityIndexing.from_model(m, "robot", device)
-  robot = EntityData(ix, sim.data, sim.model, device, frames, soft_joint_pos_limit_factor=0.9)
   key = torch.tensor(m.keys["robot/init_state"]["qpos"], dtype=torch.float32, device=dev)
   nu = len(ix.joint_names)
   t = torch.arange(frames, dtype=torch.float64, device=dev)[:, None] / fps
   # joints: one sinusoid each (0.3-0.8 Hz, staggered phases), amplitude within the soft limits about the keyframe
-  lim = robot.soft_joint_pos_limits[0].double()
+  lim = soft_limits.double()
   q0 = key[7:].double().clamp(lim[:, 0], lim[:, 1])
   # (legs swing little, so that the feet stay on the ground: RSI puts the robot in the clip's pose)
   cap = torch.tensor([0.04 if any(s in nm for s in ("hip", "knee", "ankle")) else 0.35 for nm in ix.joint_names],
@@ -58,19 +56,17 @@ def make_clip(path, frames: int = 960, fps: float = 50.0, device: str = "cuda:0"
   lin[:, 2] = bob * wb * torch.cos(wb * t[:, 0])
   ang_w = torch.zeros(frames, 3, device=dev)
   ang_w[:, 2] = wz
-  d = sim.data
-  d.qpos[:] = torch.cat([pos.float(), quat, jp.float()], dim=1)
-  d.qvel[:] = torch.cat([lin.float(), quat_apply_inverse(quat, ang_w), jv.float()], dim=1)  # free joint: body-frame angular velocity
-  sim.forward()
-  pose, vel = robot.body_link_pose_w, robot.body_link_vel_w
+  return pos.float(), quat, lin.float(), ang_w, jp.float(), jv.float()
 
-  def host(x):
-    return x.detach().to("cpu", torch.float32).numpy().copy()
 
-  np.savez(path, fps=np.array([fps]), joint_pos=host(d.qpos[:, 7:]), joint_vel=host(d.qvel[:, 6:]),
-           body_pos_w=host(pose[..., 0:3]), body_quat_w=host(pose[..., 3:7]), body_lin_vel_w=host(vel[..., 0:3]),
-           body_ang_vel_w=host(vel[..., 3:6]))
-  return str(path)
+def make_clip(path, frames: int = 960, fps: float = 50.0, device: str = "cuda:0", sim=None, model=None) -> str:
+  m = model if model is not None else load_compiled("g1_tracking_flat")
+  if sim is None:
+    sim = Simulation(frames, SimulationCfg(), m, device)
+  ix = EntityIndexing.from_model(m, "robot", device)
+  robot = EntityData(ix, sim.data, sim.model, device, frames, soft_joint_pos_limit_factor=0.9)
+  motion = motion_law(m, ix, robot.soft_joint_pos_limits[0], frames, fps, device)
+  return record_motion(sim, robot, *motion, fps, path)
 
 
 if __name__ == "__main__":
